@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- queries/sec of the Infidex search path on B200 (BASELINE.json metric), one JSON line on rank 0.
+"""bench.py -- queries/sec of the Infidex search path on H100 (BASELINE.json metric), one JSON line on rank 0.
 
   python bench.py --gpus 1 --steps K --warmup W            # our CUDA path; default workload = the metric's own config:
                                                             # BASELINE.json configs[2], 10M multi-field docs, 10k-query batch
@@ -12,6 +12,8 @@ sample of a timed batch is answered by the oracle (CPU restatement of the refere
 `cpu_baseline` -- and the GPU's records for those queries must be identical (DocumentId order, Score bits, Tiebreaker bytes);
 a mismatch fails the run instead of printing a line.
 N > 1: see `run_ours` (one process per GPU under torchrun).
+--dump-outputs DIR: after the timed steps, the records of the last timed batch (what ifx_batch_download hands a caller) go to
+DIR/<name>.npy as float32 / float64; the corpus and the query batches are seeded, so two builds can be compared file for file.
 """
 import argparse
 import json
@@ -88,7 +90,23 @@ def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, key, score, tie, n, total_candidates, status):
+    """Writes the records of one batch as <name>.npy: the int64 DocumentIds widened to float64 (exact below 2**53), every other
+    array as float32 (counts and bytes are exact below 2**24, more than any workload's document count)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"doc_key": np.asarray(key, np.float64), "score": np.asarray(score, np.float32), "tiebreaker": np.asarray(tie, np.float32),
+              "n_records": np.asarray(n, np.float32), "total_candidates": np.asarray(total_candidates, np.float32), "status": np.asarray(status, np.float32)}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise SystemExit("--dump-outputs: %d bytes exceed the %d-byte limit" % (total, DUMP_LIMIT_BYTES))
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def make_corpus(wl):
@@ -222,6 +240,8 @@ def run_sharded(args, wl, rank, world, local):
                 agg[k] += getattr(st, k)
             if first is None:
                 first = merged
+    if args.dump_outputs and rank == 0:       # the merged records of the last timed batch (facets are merged as strings: not dumped)
+        dump_outputs(args.dump_outputs, *merged[:6])
     exch = dict(eng.exchange_ms); host = dict(eng.host_ms)
     for u in ups:
         eng.FreeBatch(u)
@@ -321,6 +341,9 @@ def run_ours(args, wl, rank, world, local):
             algo += st.algo_bytes_stage1; launches += st.kernel_launches; q_max = max(q_max, st.s1_query_ms_max); q_sum += st.s1_query_ms_sum
             s1_info = {"queries_scored_per_warp": st.s1_light + st.s1_mid, "queries_scored_per_cta": st.s1_heavy, "waves": st.s1_waves, "staging_pool_bytes": int(st.s1_pool_bytes)}
     barrier()
+    if args.dump_outputs and rank == 0:       # a device-resident batch carries no facet tables: the records are its whole output
+        b = eng.DownloadBatch(handles[-1], eng.PackBatch(batches[-1]))
+        dump_outputs(args.dump_outputs, b["keys"], b["scores"], b["ties"], b["n"], b["total"], b["status"])
     for h in handles:
         eng.FreeBatch(h)
     # ---- e2e: host buffers in / out through the C-ABI call ifx_search_batch (query upload + result download inside the region) --
@@ -350,10 +373,6 @@ def run_ours(args, wl, rank, world, local):
     peak, peak_src = measured_peak()
     s1_ms = agg["ms_stage1"] / args.steps; s1_bytes = algo / args.steps
     achieved = (s1_bytes / 1e9) / (s1_ms / 1e3) if s1_ms > 0 else 0.0
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "stage1_traffic.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp)).get(args.workload)
     clocks = None
     if clk:
         sm = sorted(c[0] for c in clk); reasons = set()
@@ -365,11 +384,11 @@ def run_ours(args, wl, rank, world, local):
     line = {"metric": "queries/sec", "value": value, "unit": "queries/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": step_ms,
             "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",      # N > 1 splits this same index and batch over N GPUs (run_sharded)
             "config": {"workload": wl["label"], "batch": wl["nq"], "filter": bool(flt), "parallelism": "1 GPU",
-                       "l2": "256 MiB L2 flush before every timed step; the index (text alone %.0f MB) also exceeds the 126 MB L2" % text_mb,
+                       "l2": "256 MiB L2 flush before every timed step; the index (text alone %.0f MB) also exceeds the 50 MB L2" % text_mb,
                        "corpus_gen_s": round(t_gen, 1), "index_build_s": round(t_index, 1), "setup_s": round(t_setup, 1), "bad_status": bad_status},
             "phases_ms_per_step": {k: round(v / args.steps, 3) for k, v in agg.items()},
             "stage1": s1_info,
-            "roofline": {"bound": "hbm", "kernel": "Stage 1 = k_select_lookup (posting streams, selection) + k_score_cta + k_score_warp + k_s1_finish", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+            "roofline": {"bound": "hbm", "kernel": "Stage 1 = k_select_lookup (posting streams, selection) + k_score_cta + k_score_warp + k_s1_finish", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "algo_bytes_per_launch": s1_bytes, "ms_per_launch": s1_ms, "peak_source": peak_src,
                          "select_lookup_ms_per_launch": agg["ms_s1_select"] / args.steps,
                          "longest_query_ms": q_max, "sum_query_ms_per_launch": q_sum / args.steps},
@@ -399,6 +418,7 @@ def main():
     ap.add_argument("--workload", default="c3", choices=list(WORKLOADS), help="default: c3 = BASELINE.json configs[2], the configuration the metric is quoted on")
     ap.add_argument("--ref-sample", type=int, default=512, help="queries per step of the CPU arms (bounded sample of the batch)")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the oracle leg (cpu_baseline + parity assertion)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the records of the last timed batch to DIR/<name>.npy")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))

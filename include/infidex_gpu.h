@@ -1,4 +1,4 @@
-/* infidex_gpu.h -- C-ABI of the Blackwell-native Infidex search path (libinfidex_gpu.so).
+/* infidex_gpu.h -- C-ABI of the H100-native Infidex search path (libinfidex_gpu.so).
  *
  * Drop-in boundary (SURVEY.md 8b): the reference (lofcz/Infidex, C#) has no FFI of its own; this ABI is what a
  * P/Invoke shim behind `SearchEngine` binds (see INTEGRATION.md):

@@ -1,4 +1,4 @@
-"""infidex_b200 -- Blackwell-native (sm_100a) search path behind the lofcz/Infidex API surface."""
+"""infidex_b200 -- H100-native (sm_90a) search path behind the lofcz/Infidex API surface."""
 from .engine import (Document, DocumentFields, Field, NativeError, Query, Result, ScoreEntry, SearchEngine, Stats, Weight)
 from .filter import Filter, FilterParseError
 

@@ -1,4 +1,4 @@
-"""Build the native libraries of infidex_b200 in-tree (sm_100a only)."""
+"""Build the native libraries of infidex_b200 in-tree (sm_90a, H100, only)."""
 import os
 import subprocess
 
@@ -7,7 +7,7 @@ CSRC = os.path.join(PKG, "csrc")
 GPU_LIB = os.path.join(PKG, "libinfidex_gpu.so")
 HOST_LIB = os.path.join(PKG, "libinfidex_host.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-fmad=false", "-std=c++17", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-fmad=false", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC"]
 GXX_FLAGS = ["-std=c++17", "-O2", "-fPIC", "-ffp-contract=off", "-shared", "-pthread"]
 

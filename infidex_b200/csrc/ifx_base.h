@@ -1,7 +1,7 @@
 // infidex_b200 -- shared POD layout + execution-context abstraction.
 //
 // The search kernels are written once against `Ctx` (a cooperative group of threads):
-//   * CUDA build (nvcc, sm_100a): Ctx == one CTA; sync() is __syncthreads, ballot() is __ballot_sync, atomics are
+//   * CUDA build (nvcc, sm_90a): Ctx == one CTA; sync() is __syncthreads, ballot() is __ballot_sync, atomics are
 //     the hardware ones. This is the product.
 //   * IFX_EMU build (g++, tests only): Ctx == one host thread (group size 1, warp size 1). Used by the CPU test
 //     suite to check the kernel *logic* against the oracle without a GPU. It is never loaded by the product.

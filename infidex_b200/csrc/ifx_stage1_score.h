@@ -145,7 +145,7 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
     // ---- 3. tf lookups
     unsigned long long cost_s = 0; int n_dict = 0;
     for (int t = 0; t < T; t++) if (sh.order[t] >= 0 && sh.terms[t].term_id >= 0) { cost_s += 5ULL * (unsigned long long)sh.terms[t].len; n_dict++; }
-    const bool forward = force_mode == 1 ? true : (force_mode == 2 ? false : (n_dict > 0 && 3ULL * (unsigned long long)n_cand * (unsigned long long)fwd_avg_bytes < cost_s));      // random forward-list reads cost ~3x a streamed byte (measured, profiles/r2)
+    const bool forward = force_mode == 1 ? true : (force_mode == 2 ? false : (n_dict > 0 && 3ULL * (unsigned long long)n_cand * (unsigned long long)fwd_avg_bytes < cost_s));      // cost model: a random forward-list read costs ~3x a streamed byte
     const S1Cont* ctab = reinterpret_cast<const S1Cont*>(ws.ctab);
     const S1Probe* probe = reinterpret_cast<const S1Probe*>(ws.probe);
     auto put_hit = [&](int d, S1Probe pv, int a, uint8_t tfv) {      // candidate d (bit set in pv.bits) of row a

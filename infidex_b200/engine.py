@@ -1,13 +1,13 @@
 """Host-side mirror of the reference's public API over the infidex_b200 C-ABI.
 
-Mirrors (names, argument meaning, error behaviour) of /root/reference/src/Infidex:
+Mirrors (names, argument meaning, error behaviour) of lofcz/Infidex, src/Infidex:
   SearchEngine.CreateDefault / IndexDocuments / Search      SearchEngine.cs:78-92, 96-106, 256-319
   Query (Text, MaxNumberOfRecordsToReturn, EnableCoverage, EnableFacets, CoverageDepth, Filter)   Api/Query.cs
   Result (Records, Facets, TotalCandidates), ScoreEntry (Score, DocumentId, Tiebreaker)            Api/Result.cs, Core/ScoreEntry.cs
   Document / DocumentFields / Field / Weight                                                       Core/Document.cs, Api/*
   Filter.Parse(...) -> INFISCRIPT-V1 bytecode (Filtering/FilterCompiler.cs, BytecodeSerializer.cs) see filter.py
 
-The search itself runs only in libinfidex_gpu.so (CUDA, sm_100a). There is no CPU fallback: constructing an engine
+The search itself runs only in libinfidex_gpu.so (CUDA, sm_90a). There is no CPU fallback: constructing an engine
 without the library or without a GPU raises. (`_gpu_lib` is a test hook used by the CPU test-suite to load the
 kernel *emulation* build; the package never selects it on its own.)
 """
@@ -361,6 +361,11 @@ class SearchEngine:
         st = stats if stats is not None else Stats()
         self._check(self._gpu.ifx_batch_run(handle, C.byref(st)), "ifx_batch_run")
         return st
+
+    def DownloadBatch(self, handle, packed):
+        """Records of the last RunBatch of `handle` into the host buffers of `packed` (PackBatch of the same queries)."""
+        self._check(self._gpu.ifx_batch_download(handle, C.byref(packed["out"])), "ifx_batch_download")
+        return packed["bufs"]
 
     def FreeBatch(self, handle):
         self._gpu.ifx_batch_free(handle)

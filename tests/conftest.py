@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def _have_gpu():
@@ -29,7 +29,7 @@ def pytest_collection_modifyitems(config, items):
     """`gpu` tests need a CUDA device: on a box without one they are skipped (never silently run on a CPU path -- there is none)."""
     if _have_gpu():
         return
-    skip = pytest.mark.skip(reason="no CUDA device (run on the B200 box with -m gpu)")
+    skip = pytest.mark.skip(reason="no CUDA device (run on an H100 with -m gpu)")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)

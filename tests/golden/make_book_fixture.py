@@ -1,14 +1,14 @@
 #!/usr/bin/env python3
 """Extract the 18-book library of the reference's faceting tests into a fixture.
 
-Source : /root/reference/src/Infidex.Tests/FacetingTests.cs, CreateBookLibrary() (:589-641): CreateBookDoc(id, title, author, year,
+Source : src/Infidex.Tests/FacetingTests.cs of the reference repository, CreateBookLibrary() (:589-641): CreateBookDoc(id, title, author, year,
          genre, description) -> fields title (High, indexable), author (Med, indexable, facetable), year (Low, not indexable,
          facetable), genre (Low, indexable, facetable), description (Med, indexable) (:643-676).
 Output : tests/golden/books.json  (list of [id, title, author, year, genre, description])
-Run here only (the GPU box has no /root/reference); the output is committed.
+Usage  : make_book_fixture.py <path to FacetingTests.cs>; the output is committed, so the tests never read the reference.
 """
 import json, os, re, sys
-src = sys.argv[1] if len(sys.argv) > 1 else "/root/reference/src/Infidex.Tests/FacetingTests.cs"
+src = sys.argv[1]
 text = open(src, encoding="utf-8-sig").read()
 body = text[text.index("private static Document[] CreateBookLibrary()"):text.index("private static Document CreateBookDoc(")]
 STR = r'"((?:[^"\\]|\\.)*)"'

@@ -1,5 +1,5 @@
 """GPU parity tests, Stage 1 (BM25 backbone): the CUDA path through the C-ABI vs the oracle, bit-exact
-(DocumentId order and float32 score bits). Run on the B200 box with `pytest -m gpu`."""
+(DocumentId order and float32 score bits). Run on an H100 with `pytest -m gpu`."""
 import numpy as np
 import pytest
 
