@@ -52,7 +52,7 @@ typedef struct ifx_docset_dict {      /* string key -> ascending doc-id list (CS
     const int32_t* doc_id;
 } ifx_docset_dict;
 
-enum { IFX_COL_FILTERABLE = 1, IFX_COL_FACETABLE = 2 };
+enum { IFX_COL_FILTERABLE = 1, IFX_COL_FACETABLE = 2, IFX_COL_SORTABLE = 4 };   /* SORTABLE: emitted because the field is Field.Sortable */
 
 typedef struct ifx_column {           /* Field.Value.ToString() dictionary-encoded per document */
     const uint16_t* name; int32_t name_len;
@@ -122,6 +122,24 @@ typedef struct ifx_query {
     int32_t enable_facets;
 } ifx_query;
 
+/* Query.EnableBoost + Query.Boosts and Query.SortBy + Query.SortAscending (ResultProcessor.ApplyBoosts / ApplySort, run after the filter
+ * and before facets and Take). Optional per-query companion of ifx_query; a zero-filled entry with sort_column = IFX_SORT_NONE is "none".
+ *   n_boosts          boosts whose Filter is not null (0 = no boosts, no re-sort by score); at most IFX_MAX_BOOSTS, more is IFX_ERR_INVALID
+ *   boost_filter[i]   ifx_filter_register id of Boost[i].Filter; an unknown id sets IFX_Q_UNSUPPORTED_OP, as an unknown filter_id does
+ *   boost_strength[i] (int)Boost[i].BoostStrength
+ *   sort_column       column index (needs ifx_column_set_order first), IFX_SORT_NONE, or IFX_SORT_ALL_NULL for a SortBy field no
+ *                     document has (every value null: the sort still runs and permutes equal values)
+ * Records of a doc-id-range SHARD get IFX_Q_UNSUPPORTED_OP (post-processing belongs after the hosts' merge); a list the device holds only
+ * in part (the short-query path returns its whole list) gets IFX_Q_OVERFLOW instead of a sorted prefix. The blank query ignores both. */
+enum { IFX_MAX_BOOSTS = 16, IFX_SORT_NONE = -1, IFX_SORT_ALL_NULL = -2 };
+typedef struct ifx_query_post {
+    int32_t n_boosts;
+    int32_t boost_filter[IFX_MAX_BOOSTS];
+    int32_t boost_strength[IFX_MAX_BOOSTS];
+    int32_t sort_column;
+    int32_t sort_ascending;
+} ifx_query_post;
+
 typedef struct ifx_batch_result {     /* caller-allocated, row-major [nq][cap] */
     int32_t cap;                      /* >= max over queries of max_results */
     int32_t facet_cap;                /* facet rows per query (0 = none) */
@@ -159,13 +177,20 @@ void ifx_params_default(ifx_params* p);
 int  ifx_index_create(const ifx_index_image* img, const ifx_params* p, ifx_index** out);
 void ifx_index_destroy(ifx_index* idx);
 int  ifx_filter_register(ifx_index* idx, const uint8_t* infiscript_v1, size_t len, int* out_filter_id);
+/* The order ResultProcessor.CompareValues gives the values of a column: rank[i] for dictionary entry i (n = dict.n), equal ranks <=>
+ * CompareTo == 0, null / missing sorts lowest. The caller computes it (the C# shim with .NET's own comparer, so culture-dependent string
+ * order never has to be decided on the device). A column may be registered again; a sort on a column without an order is IFX_ERR_INVALID. */
+int  ifx_column_set_order(ifx_index* idx, int32_t column, const int32_t* rank, int32_t n);
 
 /* host buffers in, host buffers out (the call SearchEngine.Search makes) */
 int  ifx_search_batch(ifx_index* idx, const ifx_query* q, int nq, ifx_batch_result* out, ifx_stats* st);
+/* the same with boosts / SortBy: post = [nq] or NULL (NULL is exactly ifx_search_batch) */
+int  ifx_search_batch_post(ifx_index* idx, const ifx_query* q, const ifx_query_post* post, int nq, ifx_batch_result* out, ifx_stats* st);
 
 /* split form: upload once, run on device (timed), read back */
 int  ifx_batch_upload(ifx_index* idx, const ifx_query* q, int nq, ifx_batch** out);
-int  ifx_batch_refill(ifx_batch* b, const ifx_query* q, int nq);      /* the same handle for the next batch: device buffers are kept while they fit */
+int  ifx_batch_refill(ifx_batch* b, const ifx_query* q, int nq);      /* the same handle for the next batch: device buffers are kept while they fit; clears the boosts / SortBy */
+int  ifx_batch_set_post(ifx_batch* b, const ifx_query_post* post);    /* [nq] boosts / SortBy of the uploaded queries, NULL = none; kept until the next refill */
 int  ifx_batch_run(ifx_batch* b, ifx_stats* st);
 int  ifx_batch_download(ifx_batch* b, ifx_batch_result* out);
 void ifx_batch_free(ifx_batch* b);

@@ -11,7 +11,7 @@
 extern "C" {
 #endif
 
-enum { IFX_FIELD_INDEXABLE = 1, IFX_FIELD_FILTERABLE = 2, IFX_FIELD_FACETABLE = 4 };   /* Field.Indexable / Filterable / Facetable */
+enum { IFX_FIELD_INDEXABLE = 1, IFX_FIELD_FILTERABLE = 2, IFX_FIELD_FACETABLE = 4, IFX_FIELD_SORTABLE = 8 };   /* Field.Indexable / Filterable / Facetable / Sortable */
 
 typedef struct ifx_builder ifx_builder;
 
@@ -39,6 +39,9 @@ int ifx_builder_num_columns(ifx_builder* b);
 int ifx_builder_column_name(ifx_builder* b, int c, uint16_t* buf, int cap);
 int ifx_builder_column_dict_size(ifx_builder* b, int c);
 int ifx_builder_column_value(ifx_builder* b, int c, int id, uint16_t* buf, int cap);
+/* ResultProcessor.CompareValues ranks of column c's dictionary entries (rank[ifx_builder_column_dict_size]) for ifx_column_set_order:
+ * int64 / double values compared as numbers of their own type, strings ordinally; IFX_ERR_UNSUPPORTED when the field mixes runtime types */
+int ifx_builder_column_order(ifx_builder* b, int c, int32_t* rank);
 
 #ifdef __cplusplus
 }

@@ -52,7 +52,8 @@ struct StrDict {                     // n strings + open-addressing hash (key = 
 
 struct DocsetDict { StrDict keys; const int64_t* row_ptr; const int32_t* doc_id; };
 
-struct Column { const int32_t* value_id; StrDict dict; const double* dict_num; const uint8_t* dict_is_num; int32_t flags; int32_t name_const_hash_lo; };
+struct Column { const int32_t* value_id; StrDict dict; const double* dict_num; const uint8_t* dict_is_num; int32_t flags; int32_t name_const_hash_lo;
+                const int32_t* rank; };     // SortBy order per dictionary entry (ifx_column_set_order), null until registered
 
 struct DevIndex {
     int32_t n_docs, n_live; float avgdl; int32_t stop_term_limit;

@@ -194,6 +194,7 @@ struct ifx_builder {
     // documents (columnar, appended per add_docs call)
     std::vector<int64_t> keys; std::vector<std::vector<str>> values;   // values[f][d] = ToString(), kind 0 -> null flag
     std::vector<std::vector<uint8_t>> is_null;
+    std::vector<int> kind;                                             // per field: runtime type of its values (add_docs kinds), 0 none yet, -1 mixed
     // image storage
     ifx_index_image img{}; bool finished = false;
     std::vector<uint8_t> deleted; std::vector<float> doc_len; std::vector<char16_t> text; std::vector<int64_t> text_off;
@@ -204,6 +205,7 @@ struct ifx_builder {
     std::vector<uint16_t> champ_chars; std::vector<int32_t> champ_off, champ_doc; std::vector<float> champ_score;
     std::vector<int32_t> raw_doc; std::vector<char16_t> raw_chars; std::vector<int64_t> raw_off;
     std::vector<ifx_column> cols; std::vector<std::vector<int32_t>> col_ids; std::vector<std::vector<char16_t>> col_chars; std::vector<std::vector<uint32_t>> col_off; std::vector<str> col_names;
+    std::vector<int> col_kind;                                         // kind of the column's field
 };
 
 static float compute_idf_host(int total, int df) {   // Bm25Scorer.ComputeIdf
@@ -217,7 +219,7 @@ extern "C" {
 ifx_builder* ifx_builder_create(int nfields, const uint16_t* names, const int32_t* name_off, const int32_t* weight, const int32_t* flags) {
     ifx_builder* b = new ifx_builder();
     for (int i = 0; i < nfields; i++) b->schema.push_back({str((const char16_t*)names + name_off[i], name_off[i + 1] - name_off[i]), weight[i], flags[i]});
-    b->values.resize(nfields); b->is_null.resize(nfields);
+    b->values.resize(nfields); b->is_null.resize(nfields); b->kind.assign(nfields, 0);
     return b;
 }
 void ifx_builder_destroy(ifx_builder* b);
@@ -226,6 +228,7 @@ int ifx_builder_add_docs(ifx_builder* b, int n, const int64_t* keys, const int32
     if (b->finished) return IFX_ERR_INVALID;
     int F = (int)b->schema.size();
     b->keys.insert(b->keys.end(), keys, keys + n);
+    for (int f = 0; f < F; f++) if (kinds[f] != 0) b->kind[f] = (b->kind[f] == 0 || b->kind[f] == kinds[f]) ? kinds[f] : -1;
     const int hw = (int)std::max(1u, std::min(std::thread::hardware_concurrency(), 64u));
     for (int f = 0; f < F; f++) { auto& v = b->values[f]; auto& nl = b->is_null[f]; const size_t base = v.size(); v.resize(base + n); nl.resize(base + n, kinds[f] == 0 ? 1 : 0);
         if (kinds[f] != 0) par_for(n, n >= 100000 ? hw : 1, [&, f](int64_t a, int64_t e, int) { for (int64_t d = a; d < e; d++) v[base + d] = value_to_string(kinds[f], cols[f], offs ? offs[f] : nullptr, (int)d); }); }
@@ -341,10 +344,10 @@ int ifx_builder_finish(ifx_builder* b, int threads) {
           b->affix_chars.assign(g.arena.begin(), g.arena.end()); if (b->affix_chars.empty()) b->affix_chars.push_back(0); b->affix_off = g.off; if (b->affix_last.empty()) b->affix_last.push_back(0); }
         // filter / facet columns
         for (int f = 0; f < F; f++) {
-            if (!(b->schema[f].flags & (IFX_FIELD_FILTERABLE | IFX_FIELD_FACETABLE))) continue;
+            if (!(b->schema[f].flags & (IFX_FIELD_FILTERABLE | IFX_FIELD_FACETABLE | IFX_FIELD_SORTABLE))) continue;
             Interner g; std::vector<int32_t> ids(N);
             for (int d = 0; d < N; d++) ids[d] = b->is_null[f][d] ? -1 : g.intern(b->values[f][d]);
-            b->col_ids.push_back(std::move(ids)); b->col_chars.emplace_back(g.arena.begin(), g.arena.end()); if (b->col_chars.back().empty()) b->col_chars.back().push_back(0); b->col_off.push_back(g.off); b->col_names.push_back(b->schema[f].name);
+            b->col_ids.push_back(std::move(ids)); b->col_chars.emplace_back(g.arena.begin(), g.arena.end()); if (b->col_chars.back().empty()) b->col_chars.back().push_back(0); b->col_off.push_back(g.off); b->col_names.push_back(b->schema[f].name); b->col_kind.push_back(b->kind[f]);
         }
     };
     {   // the four keyed-record sets merge independently; the small dictionaries (word idf, affix words, columns) alongside
@@ -376,8 +379,9 @@ int ifx_builder_finish(ifx_builder* b, int threads) {
     float avgdl = N > 0 ? total / (float)N : 0.f;
     stage("doc lengths");
     b->cols.resize(b->col_ids.size());
-    { int ci = 0; for (int f = 0; f < F; f++) { if (!(b->schema[f].flags & (IFX_FIELD_FILTERABLE | IFX_FIELD_FACETABLE))) continue; ifx_column& c = b->cols[ci];
-        c.name = (const uint16_t*)b->col_names[ci].data(); c.name_len = (int)b->col_names[ci].size(); c.flags = ((b->schema[f].flags & IFX_FIELD_FILTERABLE) ? IFX_COL_FILTERABLE : 0) | ((b->schema[f].flags & IFX_FIELD_FACETABLE) ? IFX_COL_FACETABLE : 0);
+    { int ci = 0; for (int f = 0; f < F; f++) { if (!(b->schema[f].flags & (IFX_FIELD_FILTERABLE | IFX_FIELD_FACETABLE | IFX_FIELD_SORTABLE))) continue; ifx_column& c = b->cols[ci];
+        c.name = (const uint16_t*)b->col_names[ci].data(); c.name_len = (int)b->col_names[ci].size(); c.flags = ((b->schema[f].flags & IFX_FIELD_FILTERABLE) ? IFX_COL_FILTERABLE : 0) | ((b->schema[f].flags & IFX_FIELD_FACETABLE) ? IFX_COL_FACETABLE : 0)
+            | (!(b->schema[f].flags & (IFX_FIELD_FILTERABLE | IFX_FIELD_FACETABLE)) ? IFX_COL_SORTABLE : 0);
         c.value_id = b->col_ids[ci].data(); c.dict = {(const uint16_t*)b->col_chars[ci].data(), b->col_off[ci].data(), (int)b->col_off[ci].size() - 1}; ci++; } }
     stage("columns");
     // ---- image
@@ -532,4 +536,27 @@ extern "C" int ifx_builder_column_name(ifx_builder* b, int c, uint16_t* buf, int
 extern "C" int ifx_builder_column_dict_size(ifx_builder* b, int c) { return (int)b->col_off[c].size() - 1; }
 extern "C" int ifx_builder_column_value(ifx_builder* b, int c, int id, uint16_t* buf, int cap) {
     uint32_t o = b->col_off[c][id], e = b->col_off[c][id + 1]; int n = (int)std::min<size_t>(e - o, (size_t)cap); std::memcpy(buf, b->col_chars[c].data() + o, (size_t)n * 2); return (int)(e - o);
+}
+
+// ResultProcessor.CompareValues over the distinct values of column c, from the field's own runtime type: int64 as int64 (the dictionary holds
+// the exact decimal text), double as double (shortest round-trip text; double.CompareTo: NaN lowest, -0 == 0), strings ordinally (this
+// project's restatement of the culture-dependent string.CompareTo; a C# host ranks with .NET's own comparer instead). Dense ranks from 0.
+extern "C" int ifx_builder_column_order(ifx_builder* b, int c, int32_t* rank) {
+    if (!b || !b->finished || !rank || c < 0 || c >= (int)b->col_off.size()) return IFX_ERR_INVALID;
+    const int kind = b->col_kind[c]; if (kind < 0) return IFX_ERR_UNSUPPORTED;      // values of several runtime types: no total order
+    const int n = (int)b->col_off[c].size() - 1;
+    auto at = [&](int i) { return sv(b->col_chars[c].data() + b->col_off[c][i], b->col_off[c][i + 1] - b->col_off[c][i]); };
+    auto ascii = [&](int i, char* buf) { sv v = at(i); size_t m = std::min<size_t>(v.size(), 63); for (size_t k = 0; k < m; k++) buf[k] = (char)v[k]; return m; };
+    std::vector<int64_t> iv; std::vector<double> dv;
+    if (kind == 2) { iv.resize(n); for (int i = 0; i < n; i++) { char buf[64]; size_t m = ascii(i, buf); std::from_chars(buf, buf + m, iv[i]); } }
+    if (kind == 3) { dv.resize(n); for (int i = 0; i < n; i++) { char buf[64]; size_t m = ascii(i, buf); std::from_chars(buf, buf + m, dv[i]); } }
+    auto cmp = [&](int x, int y) -> int {
+        if (kind == 2) return iv[x] < iv[y] ? -1 : (iv[x] > iv[y] ? 1 : 0);
+        if (kind == 3) { double a = dv[x], e = dv[y]; if (a < e) return -1; if (a > e) return 1; if (a == e) return 0; return std::isnan(a) ? (std::isnan(e) ? 0 : -1) : 1; }
+        sv a = at(x), e = at(y); return a < e ? -1 : (a > e ? 1 : 0);
+    };
+    std::vector<int32_t> ord(n); std::iota(ord.begin(), ord.end(), 0);
+    std::sort(ord.begin(), ord.end(), [&](int x, int y) { return cmp(x, y) < 0; });
+    for (int i = 0, r = 0; i < n; i++) { if (i > 0 && cmp(ord[i - 1], ord[i]) != 0) r++; rank[ord[i]] = r; }
+    return IFX_OK;
 }

@@ -395,11 +395,11 @@ IFX_FN int64_t compact_bits(const Ctx& c, const DevIndex& ix, S1Workspace& ws, S
     return total;
 }
 
-// .NET ArraySortHelper<T>.IntrospectiveSort with comparison (b.Idf.CompareTo(a.Idf)) over term indices -- unstable,
-// reproduced exactly because idf ties decide which lists the selector unions (TieredCandidateSelector.cs:128,253).
-struct IdfSorter {
-    const TermS* t;
-    IFX_FN int cmp(int a, int b) const { float x = t[b].idf, y = t[a].idf; return x < y ? -1 : (x > y ? 1 : 0); }
+// .NET ArraySortHelper<T>.IntrospectiveSort(keys, Comparison<T>) over element indices -- unstable, reproduced exactly because the tie
+// order is observable: idf ties decide which lists the selector unions (TieredCandidateSelector.cs:128,253), and score / SortBy ties decide
+// the record order after boosts and sorts (ResultProcessor.cs ApplyBoosts / ApplySort). Cmp(a, b) compares the elements a and b.
+template <class Cmp> struct IntroSort {
+    Cmp cmp;
     IFX_FN void swap_if_greater(int* k, int i, int j) const { if (cmp(k[i], k[j]) > 0) { int x = k[i]; k[i] = k[j]; k[j] = x; } }
     IFX_FN void insertion(int* k, int n) const { for (int i = 0; i < n - 1; i++) { int t2 = k[i + 1]; int j = i; while (j >= 0 && cmp(t2, k[j]) < 0) { k[j + 1] = k[j]; j--; } k[j + 1] = t2; } }
     IFX_FN void down_heap(int* k, int i, int n) const { int d = k[i - 1]; while (i <= n / 2) { int ch = 2 * i; if (ch < n && cmp(k[ch - 1], k[ch]) < 0) ch++; if (!(cmp(d, k[ch - 1]) < 0)) break; k[i - 1] = k[ch - 1]; i = ch; } k[i - 1] = d; }
@@ -437,6 +437,11 @@ struct IdfSorter {
         }
     }
 };
+struct IdfCmp {      // b.Idf.CompareTo(a.Idf)
+    const TermS* t;
+    IFX_FN int operator()(int a, int b) const { float x = t[b].idf, y = t[a].idf; return x < y ? -1 : (x > y ? 1 : 0); }
+};
+using IdfSorter = IntroSort<IdfCmp>;
 
 // .NET PriorityQueue<int,float> (4-ary min-heap) on shared arrays -- Bm25Scorer.UpdateTopK (Bm25Scorer.cs:654-670)
 IFX_FN float kv_score(unsigned long long kv) {
@@ -658,7 +663,7 @@ IFX_FN int stage1_select(const Ctx& c, const DevIndex& ix, const QueryPlan& p, c
         if (c.tid() == 0) {
             bool typo = false; float max_idf = 0.f;
             for (int i = 0; i < T; i++) { if (sh.terms[i].df < 10) typo = true; if (sh.terms[i].idf > max_idf) max_idf = sh.terms[i].idf; sh.order[i] = i; }
-            IdfSorter srt{sh.terms}; srt.sort(sh.order, T);
+            IdfSorter srt{{sh.terms}}; srt.sort(sh.order, T);
             sh.bcast[0] = (typo || T == 1) ? 1 : 0; ((float*)sh.bcast)[1] = max_idf;
         }
         c.sync();

@@ -9,6 +9,7 @@
 #pragma once
 #include "ifx_stage1.h"
 #include "ifx_cov.h"
+#include "../../include/infidex_gpu.h"
 
 namespace ifx {
 
@@ -333,8 +334,61 @@ struct FinShared {
     };
 };
 
+// ---- ResultProcessor.ApplyBoosts / ApplySort (ResultProcessor.cs) over the filtered records sh.keep_*[0, nk): every (record, boost) pair
+// runs the filter VM on its own thread, the strengths are summed per record, Score + totalBoost is one float add; then the .NET introsort is
+// replayed on one thread, over record indices, first by boosted score (b.Score.CompareTo(a.Score), whenever a boost had a filter), then by
+// the caller-registered rank of the SortBy value (null lowest). Facets, TotalCandidates and Take follow on the permuted list.
+struct ScoreDescCmp {
+    const float* s;
+    IFX_FN int operator()(int a, int b) const { float x = s[b], y = s[a]; return x < y ? -1 : (x > y ? 1 : 0); }
+};
+struct RankCmp {      // CompareValues(a, b) ascending, CompareValues(b, a) descending
+    const int32_t* r; int asc;
+    IFX_FN int operator()(int a, int b) const { int x = asc ? r[a] : r[b], y = asc ? r[b] : r[a]; return x < y ? -1 : (x > y ? 1 : 0); }
+};
+IFX_FN float add_boost(float score, int total) {
+#ifdef IFX_EMU
+    return score + (float)total;
+#else
+    return __fadd_rn(score, (float)total);
+#endif
+}
+IFX_FN void post_process(const Ctx& c, const DevIndex& ix, const ifx_query_post& P, const FilterProg* filters, FinShared& sh, int nk) {
+    const int NT = c.nthreads(); const int nb = P.n_boosts; const bool sort = P.sort_column != IFX_SORT_NONE;
+    int32_t* acc = sh.pos; int32_t* perm = sh.idx;       // (free once the records are compacted into sh.keep_*)
+    if (nb > 0) {
+        for (int i = c.tid(); i < nk; i += NT) acc[i] = 0;
+        c.sync();
+        bool unsup = false;
+        for (int it = c.tid(); it < nk * nb; it += NT) { const int i = it / nb, k = it - i * nb;
+            if (filter_exec(ix, filters[P.boost_filter[k]], sh.keep_doc[i], unsup)) atomic_add(&acc[i], P.boost_strength[k]); }
+        if (unsup) sh.bcast[5] = 1;
+        c.sync();
+        for (int i = c.tid(); i < nk; i += NT) if (acc[i] > 0) sh.keep_score[i] = add_boost(sh.keep_score[i], acc[i]);
+        c.sync();
+    }
+    if (sort) {
+        const int col = P.sort_column;
+        for (int i = c.tid(); i < nk; i += NT) { int r = -1;
+            if (col >= 0) { const Column& C = ix.columns[col]; const int id = C.value_id[sh.keep_doc[i]]; if (id >= 0) r = C.rank[id]; }
+            acc[i] = r; }
+    }
+    for (int i = c.tid(); i < nk; i += NT) perm[i] = i;
+    c.sync();
+    if (c.tid() == 0) {
+        if (nb > 0) { IntroSort<ScoreDescCmp> s{{sh.keep_score}}; s.sort(perm, nk); }
+        if (sort) { IntroSort<RankCmp> s{{acc, P.sort_ascending ? 1 : 0}}; s.sort(perm, nk); }
+    }
+    c.sync();
+    for (int i = c.tid(); i < nk; i += NT) { const int j = perm[i]; sh.fv[i] = sh.keep_doc[j]; sh.score[i] = sh.keep_score[j]; sh.fc[i] = sh.keep_tie[j]; }
+    c.sync();
+    for (int i = c.tid(); i < nk; i += NT) { sh.keep_doc[i] = sh.fv[i]; sh.keep_score[i] = sh.score[i]; sh.keep_tie[i] = (uint8_t)sh.fc[i]; }
+    c.sync();
+}
+
+// `post`: [nq] boosts / SortBy per query, or null (no post-processing: exactly the plain search)
 IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p, const int32_t* s1_doc, const float* s1_score, int n1,
-                           const Stage2Buffers& B, const FilterProg* filters, int n_filters, FinShared& sh, const FinalOut& O, int q) {
+                           const Stage2Buffers& B, const FilterProg* filters, int n_filters, const ifx_query_post* post, FinShared& sh, const FinalOut& O, int q) {
     const int NT = c.nthreads(); const int K = p.depth; const int cap = B.ent_cap;
     const size_t eo = (size_t)q * cap;
     int mode = B.mode[q]; int status = p.status;
@@ -458,7 +512,7 @@ IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p,
         if (sh.bcast[5]) status |= 2;
         n_rec = have < want ? have : want;
     }
-    // ---- ApplyFilter (ResultProcessor.cs:56-69), facets over the filtered records, Take(max)
+    // ---- ApplyFilter (ResultProcessor.cs:56-69), ApplyBoosts / ApplySort, facets over the post-processed records, Take(max)
     if (c.tid() == 0) {
         int nk = n_rec; bool unsupported = false;
         if (browse) { /* filtered above */ }
@@ -468,6 +522,19 @@ IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p,
             nk = w;
         } else if (p.filter_id >= n_filters) status |= 2;
         if (unsupported) status |= 2;
+        sh.bcast[5] = 0; sh.bcast[6] = nk; sh.bcast[7] = status;
+    }
+    c.sync();
+    status = sh.bcast[7];
+    if (post && !browse && (post[q].n_boosts > 0 || post[q].sort_column != IFX_SORT_NONE)) {
+        const ifx_query_post& P = post[q]; bool run = true;
+        for (int k = 0; k < P.n_boosts; k++) if (P.boost_filter[k] < 0 || P.boost_filter[k] >= n_filters) { status |= 2; run = false; }      // unknown filter id
+        if (O.shard_info) { status |= 2; run = false; }                 // post-processing belongs after the hosts' merge of the shards
+        if (mode == 1 && p.short_kind != 0 && B.s1_total && B.s1_total[q] > n_rec) { status |= 4; run = false; }      // only a prefix of the short-query list is here
+        if (run) { post_process(c, ix, P, filters, sh, sh.bcast[6]); if (sh.bcast[5]) status |= 2; }
+    }
+    if (c.tid() == 0) {
+        int nk = sh.bcast[6];
         int nf = 0;
         if (p.enable_facets && O.fcap > 0 && nk > 0) {
             for (int col = 0; col < ix.n_columns; col++) {

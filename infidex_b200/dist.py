@@ -100,6 +100,8 @@ class ShardedSearchEngine:
         """Marshal + upload a batch once (bench `value`: inputs resident in HBM before the timed region); run it with SearchBatch(uploaded=...)."""
         eng = self.eng; packed = eng.PackBatch(queries); h = C.c_void_p()
         eng._check(eng._gpu.ifx_batch_upload(eng._index, packed["arr"], len(queries), C.byref(h)), "ifx_batch_upload")
+        if packed["post"] is not None:      # boosts / SortBy on shards: the device flags those queries IFX_Q_UNSUPPORTED_OP
+            eng._check(eng._gpu.ifx_batch_set_post(h, packed["post"]), "ifx_batch_set_post")
         return {"packed": packed, "h": h, "queries": queries}
 
     def FreeBatch(self, up):
@@ -127,6 +129,8 @@ class ShardedSearchEngine:
             if h is None:
                 h = C.c_void_p(); eng._check(g.ifx_batch_upload(eng._index, packed["arr"], nq, C.byref(h)), "ifx_batch_upload")
             self._cached_h = h
+            if packed.get("post") is not None:      # (a refill clears it) boosts / SortBy on shards: flagged IFX_Q_UNSUPPORTED_OP by the device
+                eng._check(g.ifx_batch_set_post(h, packed["post"]), "ifx_batch_set_post")
         st = stats if stats is not None else E.Stats()
 
         def sync():

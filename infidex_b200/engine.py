@@ -2,7 +2,8 @@
 
 Mirrors (names, argument meaning, error behaviour) of lofcz/Infidex, src/Infidex:
   SearchEngine.CreateDefault / IndexDocuments / Search      SearchEngine.cs:78-92, 96-106, 256-319
-  Query (Text, MaxNumberOfRecordsToReturn, EnableCoverage, EnableFacets, CoverageDepth, Filter)   Api/Query.cs
+  Query (Text, MaxNumberOfRecordsToReturn, EnableCoverage, EnableFacets, CoverageDepth, Filter,
+         EnableBoost, Boosts, SortBy, SortAscending)                                                  Api/Query.cs, Api/Boost.cs
   Result (Records, Facets, TotalCandidates), ScoreEntry (Score, DocumentId, Tiebreaker)            Api/Result.cs, Core/ScoreEntry.cs
   Document / DocumentFields / Field / Weight                                                       Core/Document.cs, Api/*
   Filter.Parse(...) -> INFISCRIPT-V1 bytecode (Filtering/FilterCompiler.cs, BytecodeSerializer.cs) see filter.py
@@ -27,17 +28,21 @@ class Weight:
 
 
 class Field:
-    def __init__(self, name, value=None, weight=Weight.Med, indexable=True, filterable=False, facetable=False):
+    def __init__(self, name, value=None, weight=Weight.Med, indexable=True, filterable=False, facetable=False, sortable=False):
         self.Name, self.Value, self.Weight = name, value, weight
-        self.Indexable, self.Filterable, self.Facetable = indexable, filterable, facetable
+        self.Indexable, self.Filterable, self.Facetable, self.Sortable = indexable, filterable, facetable, sortable
+
+
+def _field_flags(f):      # IFX_FIELD_* (include/infidex_host.h)
+    return (1 if f.Indexable else 0) | (2 if f.Filterable else 0) | (4 if f.Facetable else 0) | (8 if getattr(f, "Sortable", False) else 0)
 
 
 class DocumentFields:
     def __init__(self):
         self._fields = {}
 
-    def AddField(self, name, value=None, weight=Weight.Med, indexable=True, filterable=False, facetable=False):
-        f = name if isinstance(name, Field) else Field(name, value, weight, indexable, filterable, facetable)
+    def AddField(self, name, value=None, weight=Weight.Med, indexable=True, filterable=False, facetable=False, sortable=False):
+        f = name if isinstance(name, Field) else Field(name, value, weight, indexable, filterable, facetable, sortable)
         self._fields[f.Name] = f
         return self
 
@@ -62,6 +67,20 @@ class Query:
         self.EnableFacets = False
         self.CoverageDepth = 500
         self.Filter = None
+        self.EnableBoost = False
+        self.Boosts = None          # list[Boost]; applied only with EnableBoost
+        self.SortBy = None          # Field (or field name): records ordered by that field's value after the boosts
+        self.SortAscending = True
+
+
+class BoostStrength:
+    Low, Med, High = 1, 2, 3
+
+
+class Boost:
+    """Score + (int)BoostStrength for every record whose document passes `Filter` (ResultProcessor.ApplyBoosts)."""
+    def __init__(self, filter=None, strength=BoostStrength.Med):
+        self.Filter, self.BoostStrength = filter, strength
 
 
 class ScoreEntry:
@@ -104,6 +123,14 @@ class Stats(C.Structure):
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+MAX_BOOSTS, SORT_NONE, SORT_ALL_NULL = 16, -1, -2
+
+
+class _QueryPost(C.Structure):
+    _fields_ = [("n_boosts", C.c_int32), ("boost_filter", C.c_int32 * MAX_BOOSTS), ("boost_strength", C.c_int32 * MAX_BOOSTS),
+                ("sort_column", C.c_int32), ("sort_ascending", C.c_int32)]
 
 
 class _Params(C.Structure):
@@ -197,14 +224,14 @@ class SearchEngine:
         self.IndexColumns(np.array([d.DocumentKey for d in docs], np.int64), fields, cols)
 
     def IndexColumns(self, keys, schema, columns, threads=None, upload=True):
-        """Bulk form of IndexDocuments: schema = list[Field] (values ignored), columns[f] = list[str] | int64[] | float64[].
+        """Bulk form of IndexDocuments: schema = list[Field] (values ignored), columns[f] = list[str] | int64[] | float64[] | None (all null).
         upload=False stops after the host builder (image_ptr() is valid, no device is touched)."""
         self.Dispose()
         n = len(keys)
         keys = np.ascontiguousarray(keys, np.int64)
         nb, no = pack_strings([f.Name for f in schema])
         w = np.array([f.Weight for f in schema], np.int32)
-        fl = np.array([(1 if f.Indexable else 0) | (2 if f.Filterable else 0) | (4 if f.Facetable else 0) for f in schema], np.int32)
+        fl = np.array([_field_flags(f) for f in schema], np.int32)
         self._builder = self._host.ifx_builder_create(len(schema), _p(nb), _p(no.astype(np.int32)), _p(w), _p(fl))
         self._add_columns(keys, columns)
         self._finish(schema, threads, upload)
@@ -214,6 +241,8 @@ class SearchEngine:
         kinds = np.zeros(len(columns), np.int32)
         keep, cptr, optr = [], (C.c_void_p * len(columns))(), (C.c_void_p * len(columns))()
         for i, col in enumerate(columns):
+            if col is None:                       # the field is null in every document of this chunk
+                continue
             if isinstance(col, np.ndarray) and col.dtype.kind in "iu":
                 a = np.ascontiguousarray(col, np.int64); kinds[i] = 2; cptr[i] = a.ctypes.data; keep.append(a)
             elif isinstance(col, np.ndarray) and col.dtype.kind == "f":
@@ -242,7 +271,7 @@ class SearchEngine:
         self.Dispose()
         nb, no = pack_strings([f.Name for f in schema])
         w = np.array([f.Weight for f in schema], np.int32)
-        fl = np.array([(1 if f.Indexable else 0) | (2 if f.Filterable else 0) | (4 if f.Facetable else 0) for f in schema], np.int32)
+        fl = np.array([_field_flags(f) for f in schema], np.int32)
         self._builder = self._host.ifx_builder_create(len(schema), _p(nb), _p(no.astype(np.int32)), _p(w), _p(fl))
         for keys, columns in chunks:
             self._add_columns(np.ascontiguousarray(keys, np.int64), columns)
@@ -258,6 +287,7 @@ class SearchEngine:
         self._index = idx
         self._is_indexed = True
         self._filters = {}
+        self._ordered = set()       # columns whose SortBy order is registered on the device
 
     # ---- searching --------------------------------------------------------------------------------------------------
     def _prep_text(self, text):
@@ -283,6 +313,38 @@ class SearchEngine:
             self._filters[code] = fid.value
         return self._filters[code]
 
+    def _sort_column(self, sort_by):
+        """SortBy -> device column (its CompareValues order registered on first use) or SORT_ALL_NULL. The field is looked up by its exact name,
+        as Dictionary<string, Field>.GetField does; any field with a device column may be named (the reference does not require Sortable)."""
+        name = sort_by.Name if isinstance(sort_by, Field) else str(sort_by)
+        if name not in self._columns:
+            if any(f.Name == name for f in self._schema):
+                raise ValueError("SortBy field %r is neither Sortable, Filterable nor Facetable in the schema: no device column exists for it" % name)
+            return SORT_ALL_NULL        # no document has the field: every value is null
+        c = self._columns.index(name)
+        if c not in self._ordered:
+            b = C.c_void_p(self._builder); rank = np.zeros(max(self._host.ifx_builder_column_dict_size(b, c), 1), np.int32)
+            rc = self._host.ifx_builder_column_order(b, c, _p(rank))
+            if rc:
+                raise ValueError("SortBy field %r holds values of several runtime types: they have no common order" % name)
+            self._check(self._gpu.ifx_column_set_order(self._index, c, _p(rank), self._host.ifx_builder_column_dict_size(b, c)), "ifx_column_set_order")
+            self._ordered.add(c)
+        return c
+
+    def _post(self, q):
+        """ifx_query_post of one query, or None when it has neither boosts nor a SortBy (ApplyPostProcessing, ResultProcessor.cs)."""
+        boosts = [b for b in (q.Boosts or []) if b.Filter is not None] if q.EnableBoost else []
+        if not boosts and q.SortBy is None:
+            return None
+        if len(boosts) > MAX_BOOSTS:
+            raise ValueError("at most %d boosts with a filter per query" % MAX_BOOSTS)
+        p = _QueryPost(); p.n_boosts = len(boosts)
+        for k, b in enumerate(boosts):
+            p.boost_filter[k] = self._filter_id(b.Filter); p.boost_strength[k] = int(b.BoostStrength)
+        p.sort_column = SORT_NONE if q.SortBy is None else self._sort_column(q.SortBy)
+        p.sort_ascending = int(bool(q.SortAscending))
+        return p
+
     def _pack_queries(self, queries):
         texts = [self._prep_text(q.Text) for q in queries]
         arr = (_Query * len(queries))()
@@ -292,10 +354,23 @@ class SearchEngine:
             arr[i].enable_coverage = int(q.EnableCoverage); arr[i].filter_id = self._filter_id(q.Filter); arr[i].enable_facets = int(q.EnableFacets)
         return arr, texts
 
+    def _pack_post(self, queries):
+        """[nq] ifx_query_post, or None when no query boosts or sorts (then the batch is exactly the plain search)."""
+        posts = [self._post(q) for q in queries]
+        if all(p is None for p in posts):
+            return None
+        arr = (_QueryPost * len(queries))()
+        for i, p in enumerate(posts):
+            if p is None:
+                arr[i].sort_column = SORT_NONE
+            else:
+                arr[i] = p
+        return arr
+
     def PackBatch(self, queries, facet_cap=0):
         """Host-side marshalling of a batch (what the C# shim does with `fixed` pointers): returns a reusable call object."""
         nq = len(queries)
-        arr, keep = self._pack_queries(queries)
+        arr, keep = self._pack_queries(queries); post = self._pack_post(queries)
         cap = max(1, max(q.MaxNumberOfRecordsToReturn for q in queries))
         fc = facet_cap or (256 if any(q.EnableFacets for q in queries) else 0)
         out = _BatchResult(); out.cap = cap; out.facet_cap = fc
@@ -304,12 +379,15 @@ class SearchEngine:
                     fcol=np.zeros((nq, max(fc, 1)), np.int32), fval=np.zeros((nq, max(fc, 1)), np.int32), fcnt=np.zeros((nq, max(fc, 1)), np.int32), nf=np.zeros(nq, np.int32))
         out.doc_key, out.score, out.tie, out.n, out.total_candidates, out.status = _p(bufs["keys"]), _p(bufs["scores"]), _p(bufs["ties"]), _p(bufs["n"]), _p(bufs["total"]), _p(bufs["status"])
         out.facet_column, out.facet_value, out.facet_count, out.n_facets = _p(bufs["fcol"]), _p(bufs["fval"]), _p(bufs["fcnt"]), _p(bufs["nf"])
-        return {"arr": arr, "keep": keep, "nq": nq, "out": out, "bufs": bufs}
+        return {"arr": arr, "keep": keep, "nq": nq, "out": out, "bufs": bufs, "post": post}
 
     def SearchPacked(self, packed, stats=None):
         """The bare C-ABI call ifx_search_batch on pre-marshalled host buffers (host -> device -> host)."""
         st = stats if stats is not None else Stats()
-        self._check(self._gpu.ifx_search_batch(self._index, packed["arr"], packed["nq"], C.byref(packed["out"]), C.byref(st)), "ifx_search_batch")
+        if packed.get("post") is None:
+            self._check(self._gpu.ifx_search_batch(self._index, packed["arr"], packed["nq"], C.byref(packed["out"]), C.byref(st)), "ifx_search_batch")
+        else:
+            self._check(self._gpu.ifx_search_batch_post(self._index, packed["arr"], packed["post"], packed["nq"], C.byref(packed["out"]), C.byref(st)), "ifx_search_batch_post")
         return st
 
     def SearchBatch(self, queries, stats=None, facet_cap=0):
@@ -317,7 +395,7 @@ class SearchEngine:
         if not self._is_indexed:
             return [Result([], None, 0) for _ in queries]
         nq = len(queries)
-        arr, keep = self._pack_queries(queries)
+        arr, keep = self._pack_queries(queries); post = self._pack_post(queries)
         cap = max(1, max(q.MaxNumberOfRecordsToReturn for q in queries))
         fc = facet_cap or (256 if any(q.EnableFacets for q in queries) else 0)
         out = _BatchResult(); out.cap = cap; out.facet_cap = fc
@@ -327,7 +405,10 @@ class SearchEngine:
         out.doc_key, out.score, out.tie, out.n, out.total_candidates, out.status = _p(keys), _p(scores), _p(ties), _p(n), _p(total), _p(status)
         out.facet_column, out.facet_value, out.facet_count, out.n_facets = _p(fcol), _p(fval), _p(fcnt), _p(nf)
         st = stats if stats is not None else Stats()
-        self._check(self._gpu.ifx_search_batch(self._index, arr, nq, C.byref(out), C.byref(st)), "ifx_search_batch")
+        if post is None:
+            self._check(self._gpu.ifx_search_batch(self._index, arr, nq, C.byref(out), C.byref(st)), "ifx_search_batch")
+        else:
+            self._check(self._gpu.ifx_search_batch_post(self._index, arr, post, nq, C.byref(out), C.byref(st)), "ifx_search_batch_post")
         self.last_raw = (keys, scores, ties, n, total, status)
         res = []
         for i in range(nq):
@@ -352,9 +433,13 @@ class SearchEngine:
 
     # ---- device-resident batches (bench `value`: inputs already in HBM when the timed region starts) -----------------
     def UploadBatch(self, queries):
-        arr, keep = self._pack_queries(queries)
+        arr, keep = self._pack_queries(queries); post = self._pack_post(queries)
         h = C.c_void_p()
         self._check(self._gpu.ifx_batch_upload(self._index, arr, len(queries), C.byref(h)), "ifx_batch_upload")
+        if post is not None:
+            rc = self._gpu.ifx_batch_set_post(h, post)
+            if rc:
+                self._gpu.ifx_batch_free(h); self._check(rc, "ifx_batch_set_post")
         return h
 
     def RunBatch(self, handle, stats=None):
