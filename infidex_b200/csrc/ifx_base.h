@@ -1,10 +1,11 @@
 // infidex_b200 -- shared POD layout + execution-context abstraction.
 //
-// The search kernels are written once against `Ctx` (a cooperative group of threads):
+// The search kernels and their __global__ wrappers are written once against `Ctx` (a cooperative group of threads):
 //   * CUDA build (nvcc, sm_90a): Ctx == one CTA; sync() is __syncthreads, ballot() is __ballot_sync, atomics are
 //     the hardware ones. This is the product.
-//   * IFX_EMU build (g++, tests only): Ctx == one host thread (group size 1, warp size 1). Used by the CPU test
-//     suite to check the kernel *logic* against the oracle without a GPU. It is never loaded by the product.
+//   * IFX_EMU build (g++, tests only): Ctx == one host thread (group size 1, warp size 1). The kernels are host functions
+//     and the launch shim of ifx_api.inl calls them once per block, so the CPU test suite runs the product's host driver
+//     and kernels and checks them against the oracle without a GPU. It is never loaded by the product.
 #pragma once
 #include <stdint.h>
 #include <stddef.h>
@@ -15,9 +16,16 @@
 #include <algorithm>
 #define IFX_FN inline
 #define IFX_FN_OUTLINED inline
-#define IFX_KERNEL_ATTR
+#define IFX_GLOBAL
+#define IFX_BOUNDS(...)
+#define IFX_SHARED static thread_local                  // static shared memory: one instance, reused by the blocks run in turn
+#define IFX_DYN_SHARED(name) unsigned char* name = ifx::emu_grid().smem
 #else
 #include <cuda_runtime.h>
+#define IFX_GLOBAL __global__
+#define IFX_BOUNDS(...) __launch_bounds__(__VA_ARGS__)
+#define IFX_SHARED __shared__
+#define IFX_DYN_SHARED(name) extern __shared__ __align__(16) unsigned char name[]
 #define IFX_FN __device__ __forceinline__
 // large helpers with several call sites inside one kernel: one shared body keeps the instruction footprint (and the i-cache
 // miss rate of divergent warps) down
@@ -124,10 +132,19 @@ IFX_FN int dict_lookup(const StrDict& d, const uint16_t* s, int n) {
 }
 
 // ---- execution context ------------------------------------------------------------------------------------------
+// block() / nblocks() are blockIdx.x / gridDim.x; gtid() / gthreads() and gwarp() / gwarps() number the threads and the warps of the
+// whole grid. A block-strided loop of a kernel wrapper adds `(unsigned)c.nthreads()`: wrap-around arithmetic like blockDim.x,
+// so nvcc emits the plain loop instead of computing a trip count.
 #ifdef IFX_EMU
+// The block the launch shim is running (one host thread per block) and its dynamic shared memory.
+struct EmuGrid { unsigned block = 0, nblocks = 1; unsigned char* smem = nullptr; };
+inline EmuGrid& emu_grid() { static thread_local EmuGrid g; return g; }
 struct Ctx {
     static constexpr int WS = 1;
+    unsigned b_ = emu_grid().block, nb_ = emu_grid().nblocks;
     int tid() const { return 0; } int nthreads() const { return 1; } int lane() const { return 0; } int warp() const { return 0; } int nwarps() const { return 1; }
+    unsigned block() const { return b_; } unsigned nblocks() const { return nb_; }
+    int64_t gtid() const { return b_; } int64_t gthreads() const { return nb_; } int64_t gwarp() const { return b_; } int64_t gwarps() const { return nb_; }
     void sync() const {}
     void sync_workers(int) const {}
     void sync_team(int) const {}
@@ -141,16 +158,22 @@ inline int atomic_add(int* p, int v) { int o = *p; *p = o + v; return o; }
 inline unsigned atomic_and(unsigned* p, unsigned v) { unsigned o = *p; *p = o & v; return o; }
 inline int atomic_min(int* p, int v) { int o = *p; if (v < o) *p = v; return o; }
 inline int atomic_max(int* p, int v) { int o = *p; if (v > o) *p = v; return o; }
+inline unsigned long long atomic_max(unsigned long long* p, unsigned long long v) { unsigned long long o = *p; if (v > o) *p = v; return o; }
 inline unsigned long long atomic_add64(unsigned long long* p, unsigned long long v) { unsigned long long o = *p; *p = o + v; return o; }
 inline int popc(unsigned v) { return __builtin_popcount(v); }
 inline int ffs32(unsigned v) { return __builtin_ffs((int)v); }
 inline int popc64(unsigned long long v) { return __builtin_popcountll(v); }
+inline int clz64(long long v) { return v ? __builtin_clzll((unsigned long long)v) : 64; }
 inline float dev_logf_exact(float x) { return std::log(x); }
+inline unsigned long long globaltimer() { return 0; }
 #else
 struct Ctx {
     static constexpr int WS = 32;
     __device__ int tid() const { return threadIdx.x; } __device__ int nthreads() const { return blockDim.x; }
     __device__ int lane() const { return threadIdx.x & 31; } __device__ int warp() const { return threadIdx.x >> 5; } __device__ int nwarps() const { return blockDim.x >> 5; }
+    __device__ unsigned block() const { return blockIdx.x; } __device__ unsigned nblocks() const { return gridDim.x; }
+    __device__ int64_t gtid() const { return (int64_t)blockIdx.x * blockDim.x + threadIdx.x; } __device__ int64_t gthreads() const { return (int64_t)gridDim.x * blockDim.x; }
+    __device__ int64_t gwarp() const { return gtid() >> 5; } __device__ int64_t gwarps() const { return gthreads() >> 5; }
     __device__ void sync() const { __syncthreads(); }
     // named barrier 1 over the `n` worker threads of a warp-specialised region (n: multiple of 32; every worker warp calls it)
     __device__ void sync_workers(int n) const { asm volatile("bar.sync 1, %0;" :: "r"(n) : "memory"); }
@@ -166,12 +189,15 @@ __device__ __forceinline__ int atomic_add(int* p, int v) { return atomicAdd(p, v
 __device__ __forceinline__ unsigned atomic_and(unsigned* p, unsigned v) { return atomicAnd(p, v); }
 __device__ __forceinline__ int atomic_min(int* p, int v) { return atomicMin(p, v); }
 __device__ __forceinline__ int atomic_max(int* p, int v) { return atomicMax(p, v); }
+__device__ __forceinline__ unsigned long long atomic_max(unsigned long long* p, unsigned long long v) { return atomicMax(p, v); }
 __device__ __forceinline__ unsigned long long atomic_add64(unsigned long long* p, unsigned long long v) { return atomicAdd(p, v); }
 __device__ __forceinline__ int popc(unsigned v) { return __popc(v); }
 __device__ __forceinline__ int ffs32(unsigned v) { return __ffs((int)v); }
 __device__ __forceinline__ int popc64(unsigned long long v) { return __popcll(v); }
+__device__ __forceinline__ int clz64(long long v) { return __clzll(v); }
 // MathF.Log on the reference host is glibc logf (<1 ulp, effectively correctly rounded); evaluate in fp64 and round once.
 __device__ __forceinline__ float dev_logf_exact(float x) { return (float)log((double)x); }
+__device__ __forceinline__ unsigned long long globaltimer() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 #endif
 
 // Bm25Scorer.ComputeIdf (src/Infidex/Indexing/Bm25Scorer.cs:686-695) -- table lookup, see DevIndex::idf_table

@@ -167,3 +167,19 @@ def test_emu_short_queries(emu, movie_titles, oracle_movies):
         orc = OracleEngine(); orc.index_texts(texts); e2 = ib.SearchEngine(_gpu_lib=emu); e2.IndexColumns(np.arange(len(texts)), [ib.Field("content")], [texts])
         bad = compare_search(e2, orc, ["a", "b", "x", "ab", "a b", "xx", "y z"], max_results=10)
         assert not bad, bad[:3]
+
+
+def test_emu_staging_pool_waves(emu, monkeypatch):
+    """A Stage-1 staging pool far smaller than the batch needs (1 MB, read at index creation): the batch is finished in several
+    waves -- deferred queries, counters read back and reset between waves -- with every answer still equal to the oracle's."""
+    monkeypatch.setenv("IFX_S1_POOL_MB", "1")
+    vocab = synth.make_vocab(30_000)
+    docs = synth.gen_docs(30_000, vocab)
+    qs = synth.gen_queries(150, docs, vocab)
+    schema, cols = synth.schema_and_columns(docs, False)
+    eng, orc = build_pair(docs["keys"], schema, cols, gpu_lib=emu)
+    st = ib.Stats()
+    eng.SearchBatch([ib.Query(q, 10) for q in qs], stats=st)
+    assert st.s1_waves > 1
+    assert not compare_stage1(eng, orc, qs)
+    assert not compare_search(eng, orc, qs)
