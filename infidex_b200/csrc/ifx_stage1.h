@@ -182,8 +182,7 @@ struct S1Workspace {
     int32_t* cand;         // sorted candidate ids
     int32_t* buf_a; int32_t* buf_b;   // AND-tier ping-pong arrays
     unsigned long long* surv_g;       // [CHUNK] flush survivors of one chunk when they exceed the shared staging buffer
-    int32_t* rank;         // [n_words ..): padded tf slots before container c (scratch of the tf lookups)
-    unsigned long long* probe;   // per bitset word: (bits, candidates before the word) -- S1Probe, valid between the compaction and the tf lookups; bits all zero between queries
+    int32_t* loff;         // [n_cont + 1][streamed lists] offset of the first posting of each streamed list in container c (scratch of the tf lookups)
     int32_t* cstart;       // [n_cont + 1] candidates before container c
     int32_t* cfirst;       // [n_cont + 1] chunks before container c
     int32_t* ctab;         // [n_cont] packed S1Cont records (16 bytes each) for the tf lookups
@@ -211,6 +210,15 @@ struct S1SelShared {
     ScanTmp scan; ScanTmp scan2[2];
     int bcast[8]; long long bcast64[4];
     unsigned long long streamed_mask[2];   // terms whose list the selector streamed in full (roofline accounting)
+};
+// ... plus the tf lookups' window on one 65 536-doc container of the candidate bitset (the selection / lookup kernel only)
+constexpr int CONT_WORDS = 2048;        // bitset words per container
+struct S1LookupShared : S1SelShared {
+    alignas(16) unsigned win[CONT_WORDS];   // the container's candidate bits
+    uint16_t wrank[CONT_WORDS];             // candidates of the container before each word (<= 65 504)
+    int32_t sterm[MAX_TERMS];               // streamed list -> term
+    int32_t rlo[MAX_TERMS], rhi[MAX_TERMS]; // postings of each streamed list inside the container
+    int32_t rpre[MAX_TERMS + 1];            // the short ranges concatenated: where each list's range starts in the block-wide range (long ranges: length 0)
 };
 // ... plus what the block-wide scorer and the LD1 expansion need
 struct S1Shared : S1SelShared {

@@ -22,7 +22,6 @@ struct S1Rec {
     int32_t K, path, pad;
 };
 struct S1Queues { int32_t* light; int32_t* mid; int32_t* heavy; };
-struct alignas(8) S1Probe { unsigned bits; int32_t rank; };                     // one candidate-bitset word and the candidates before it: a posting's probe is ONE 8-byte load
 struct alignas(16) S1Cont { int32_t cstart, cnt, cpad, cfirst; };                // per container: candidates before it, its candidates, padded tf slots before it, chunks before it                           // query ids appended by stage1_lookup (counters in BatchCounters)
 
 IFX_FN int pad16(int x) { return (x + 15) & ~15; }
@@ -37,12 +36,13 @@ constexpr int W_K = 512;             // heap capacity kept in shared memory per 
 
 // ---------------------------------------------------------------------------------------------------------------
 // stage1_lookup: called right after stage1_select by the same CTA. Candidates are the bits of ws.bits.
-//   1. count + expand the bitset into the pool (ascending ids), building the rank directory (doc -> candidate index in O(1))
+//   1. count + expand the bitset into the pool (ascending ids), candidates before every container
 //   2. document lengths, deleted flags, chunk table
-//   3. tf of every (term, candidate): either every posting list streamed once against the candidate bitset (coalesced; the byte
-//      volume SURVEY 8d calls algorithmic), or -- few candidates relative to the lists -- one forward-index read per candidate
-//   4. bitset cleared again
-IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, int path, int q, S1Workspace& ws, S1SelShared& sh, S1Rec* recs,
+//   3. tf of every (term, candidate): either the posting lists streamed container by container against a shared-memory window of
+//      the candidate bitset (coalesced; only containers that hold candidates), or -- few candidates relative to the lists -- one
+//      forward-index read per candidate
+//   4. bitset cleared again (in the container walk, or here when nothing was streamed)
+IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, int path, int q, S1Workspace& ws, S1LookupShared& sh, S1Rec* recs,
                           unsigned char* spool, unsigned long long spool_cap, S1Queues queues, BatchCounters* bc, Stage1Out out, int fwd_avg_bytes, int force_mode) {
     S1Rec& rec = recs[q]; const int NT = c.nthreads(), NW = c.nwarps(); constexpr int WS = Ctx::WS;
 #if !defined(IFX_EMU) && defined(IFX_S1_TIMERS)
@@ -62,25 +62,24 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
         for (int u = 0; u < 4; u++) mycnt += popc(v[u]);
     }
     int n_cand; int ex0 = block_excl_scan(c, mycnt, sh.scan, n_cand); const int wbase = c.shfl(ex0, 0);
-    auto clear_bits = [&]() {
-        S1Probe* pr = reinterpret_cast<S1Probe*>(ws.probe);
-        for (int64_t w = c.tid(); w < nwords; w += NT) if (sh.dirty[w >> 11]) { ws.bits[w] = 0u; pr[w].bits = 0u; }
+    auto clear_bits = [&](bool words) {      // words == false: the container walk of the tf lookups has zeroed them already
+        if (words) for (int64_t w = c.tid(); w < nwords; w += NT) if (sh.dirty[w >> 11]) ws.bits[w] = 0u;
         c.sync();
         for (int k = c.tid(); k < ncont; k += NT) sh.dirty[k] = 0;
         c.sync();
     };
-    if (n_cand == 0) { clear_bits(); if (c.tid() == 0) { rec.state = 0; rec.n_cand = 0; rec.K = p.depth; rec.path = path; if (out.dbg) out.dbg[0] = 0; } c.sync(); return; }
+    if (n_cand == 0) { clear_bits(true); if (c.tid() == 0) { rec.state = 0; rec.n_cand = 0; rec.K = p.depth; rec.path = path; if (out.dbg) out.dbg[0] = 0; } c.sync(); return; }
     auto pool_alloc = [&](unsigned long long bytes) -> long long {      // block-uniform result; -1: does not fit now, -2: can never fit
         if (c.tid() == 0) { long long r; bytes = (bytes + 255ULL) & ~255ULL;
             if (bytes > spool_cap) r = -2; else { unsigned long long at = atomic_add64(&bc->s1_pool_used, bytes); r = at + bytes <= spool_cap ? (long long)at : -1; }
             sh.bcast64[2] = r; }
         c.sync(); long long r = sh.bcast64[2]; c.sync(); return r;
     };
-    auto give_up = [&](long long why) { clear_bits(); if (c.tid() == 0) { rec.state = why == -2 ? -1 : 2; rec.n_cand = n_cand; rec.K = p.depth; rec.path = path; if (why != -2) atomic_add(&bc->s1_deferred, 1); else out.n[0] = -1; } c.sync(); };      // a query larger than the whole pool is an overflow, like every other fixed buffer
+    auto give_up = [&](long long why) { clear_bits(true); if (c.tid() == 0) { rec.state = why == -2 ? -1 : 2; rec.n_cand = n_cand; rec.K = p.depth; rec.path = path; if (why != -2) atomic_add(&bc->s1_deferred, 1); else out.n[0] = -1; } c.sync(); };      // a query larger than the whole pool is an overflow, like every other fixed buffer
     const long long a1 = pool_alloc(8ULL * (unsigned long long)n_cand + 64);
     if (a1 < 0) { give_up(a1); return; }
     int32_t* cand = reinterpret_cast<int32_t*>(spool + a1); float* dlp = reinterpret_cast<float*>(spool + a1 + (((long long)n_cand * 4 + 31) & ~31LL));
-    // ---- 1b. expand + rank directory + candidates before every container
+    // ---- 1b. expand + candidates before every container
     {   int run = wbase;
         for (int64_t gb = w0; gb < w1; gb += 4 * WS) {          // four groups per trip: their words are loaded together, then scanned one after the other
             unsigned vv[4];
@@ -91,7 +90,7 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
                 const int64_t w = g0 + c.lane(); unsigned v = vv[u]; const int pc = popc(v); int incl = pc;
                 for (int d = 1; d < WS; d <<= 1) { int o = c.shfl(incl, c.lane() >= d ? c.lane() - d : 0); if (c.lane() >= d) incl += o; }
                 int o = run + incl - pc;
-                if (w < w1) { S1Probe pv; pv.bits = v; pv.rank = o; reinterpret_cast<S1Probe*>(ws.probe)[w] = pv; if ((w & 2047) == 0) ws.cstart[w >> 11] = o; }
+                if (w < w1 && (w & 2047) == 0) ws.cstart[w >> 11] = o;
                 while (v) { int b = ffs32(v) - 1; v &= v - 1; cand[o++] = (int32_t)((w << 5) | b); }
                 run += c.shfl(incl, WS - 1);
             }
@@ -99,7 +98,7 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
         if (c.tid() == 0) ws.cstart[ncont] = n_cand;
     }
     c.sync();
-    IFX_LTICK(0);   // count + expand + rank directory
+    IFX_LTICK(0);   // count + expand
     // ---- 2. lengths, deleted flags (folded into the id), chunk table
     const bool any_deleted = ix.n_live != ix.n_docs;
     for (int i0 = c.tid(); i0 < n_cand; i0 += 8 * NT) {
@@ -118,13 +117,13 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
         const int cc = c0 + c.tid(); const int cntc = cc < ncont ? ws.cstart[cc + 1] - ws.cstart[cc] : 0;
         const int nch = (cntc + CHUNK - 1) / CHUNK; const int slots = (cntc / CHUNK) * CHUNK + pad16(cntc % CHUNK);
         int t1, t2; const int e1 = block_excl_scan(c, nch, sh.scan, t1); const int e2 = block_excl_scan(c, slots, sh.scan, t2);
-        if (cc < ncont) { ws.cfirst[cc] = n_chunks + e1; ws.rank[nwords + cc] = n_slots + e2;      // padded slots before container cc: kept behind the rank directory
+        if (cc < ncont) { ws.cfirst[cc] = n_chunks + e1;
                           S1Cont ct; ct.cstart = ws.cstart[cc]; ct.cnt = cntc; ct.cpad = n_slots + e2; ct.cfirst = n_chunks + e1; reinterpret_cast<S1Cont*>(ws.ctab)[cc] = ct; }
         if (cntc > 0) atomic_max(&sh.bcast[1], cntc < CHUNK ? cntc : CHUNK);
         n_chunks += t1; n_slots += t2;
     }
     c.sync();
-    const int max_cnt = sh.bcast[1]; const int32_t* cpad = ws.rank + nwords;
+    const int max_cnt = sh.bcast[1]; const S1Cont* ctab = reinterpret_cast<const S1Cont*>(ws.ctab);
     const unsigned long long tf_bytes = (unsigned long long)(Ta > 0 ? Ta : 1) * (unsigned long long)n_slots;
     const unsigned long long chunk_bytes = ((unsigned long long)n_chunks * sizeof(S1Chunk) + 15ULL) & ~15ULL, term_bytes = (unsigned long long)(Ta > 0 ? Ta : 1) * sizeof(S1TermP);
     const long long a2 = pool_alloc(chunk_bytes + term_bytes + tf_bytes + 64);
@@ -133,7 +132,7 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
     uint8_t* tfb = spool + a2 + chunk_bytes + term_bytes;
     for (int cc = c.tid(); cc < ncont; cc += NT) {
         const int cntc = ws.cstart[cc + 1] - ws.cstart[cc]; const int nch = (cntc + CHUNK - 1) / CHUNK;
-        for (int s = 0; s < nch; s++) { S1Chunk ch; ch.start = ws.cstart[cc] + s * CHUNK; ch.cnt = cntc - s * CHUNK < CHUNK ? cntc - s * CHUNK : CHUNK; ch.tf_off = (int64_t)Ta * (cpad[cc] + s * CHUNK); chunks[ws.cfirst[cc] + s] = ch; }
+        for (int s = 0; s < nch; s++) { S1Chunk ch; ch.start = ws.cstart[cc] + s * CHUNK; ch.cnt = cntc - s * CHUNK < CHUNK ? cntc - s * CHUNK : CHUNK; ch.tf_off = (int64_t)Ta * (ctab[cc].cpad + s * CHUNK); chunks[ws.cfirst[cc] + s] = ch; }
     }
     for (int t = c.tid(); t < T; t += NT) if (sh.order[t] >= 0) { S1TermP tp; tp.idf = sh.terms[t].idf; tp.max_score = sh.terms[t].max_score; tp.suffix_after = sh.terms[t].suffix_after; tp.pad = 0; tparams[sh.order[t]] = tp; }
     {   // zero the tf matrix (16-byte stores; the block is 16-byte aligned and padded)
@@ -146,47 +145,6 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
     unsigned long long cost_s = 0; int n_dict = 0;
     for (int t = 0; t < T; t++) if (sh.order[t] >= 0 && sh.terms[t].term_id >= 0) { cost_s += 5ULL * (unsigned long long)sh.terms[t].len; n_dict++; }
     const bool forward = force_mode == 1 ? true : (force_mode == 2 ? false : (n_dict > 0 && 3ULL * (unsigned long long)n_cand * (unsigned long long)fwd_avg_bytes < cost_s));      // cost model: a random forward-list read costs ~3x a streamed byte
-    const S1Cont* ctab = reinterpret_cast<const S1Cont*>(ws.ctab);
-    const S1Probe* probe = reinterpret_cast<const S1Probe*>(ws.probe);
-    auto put_hit = [&](int d, S1Probe pv, int a, uint8_t tfv) {      // candidate d (bit set in pv.bits) of row a
-        const unsigned bit = 1u << (d & 31); const int idx = pv.rank + popc(pv.bits & (bit - 1)); const S1Cont ct = ctab[d >> 16];
-        const int jc = idx - ct.cstart, sub = jc / CHUNK; const int cnt_k = ct.cnt - sub * CHUNK < CHUNK ? ct.cnt - sub * CHUNK : CHUNK;
-        tfb[(int64_t)Ta * (ct.cpad + sub * CHUNK) + (int64_t)a * pad16(cnt_k) + (jc - sub * CHUNK)] = tfv;
-    };
-    auto stream_term = [&](const TermS& tm, int a) {      // every posting of one list against the candidate bitset
-        const int64_t len = tm.len; int64_t done = 0;
-#ifndef IFX_EMU
-        if (len >= 2048) {
-            // aligned middle of the list: 16 postings per thread in flight (four 16-byte id loads + four 4-byte tf loads), then their
-            // 16 bitset probes, then the hits
-            const int64_t pre = (int64_t)((0 - (reinterpret_cast<uintptr_t>(tm.docs) >> 2)) & 3);
-            for (int64_t i = c.tid(); i < pre; i += NT) { const int d = tm.docs[i]; const S1Probe wv = probe[d >> 5]; if ((wv.bits >> (d & 31)) & 1u) put_hit(d, wv, a, tm.tf ? tm.tf[i] : (uint8_t)1); }
-            const int4* p4 = reinterpret_cast<const int4*>(tm.docs + pre); const unsigned* t4 = tm.tf ? reinterpret_cast<const unsigned*>(tm.tf + pre) : nullptr;
-            const int64_t n4 = (len - pre) >> 2;
-            for (int64_t g0 = c.tid(); g0 < n4; g0 += 4LL * NT) {
-                int4 dv[4]; unsigned tw[4]; S1Probe wv[16];
-#pragma unroll
-                for (int u = 0; u < 4; u++) { const int64_t g = g0 + (int64_t)u * NT; if (g < n4) { dv[u] = p4[g]; tw[u] = t4 ? t4[g] : 0x01010101u; } else { dv[u] = make_int4(-1, -1, -1, -1); tw[u] = 0u; } }
-#pragma unroll
-                for (int u = 0; u < 4; u++) { const int dd[4] = {dv[u].x, dv[u].y, dv[u].z, dv[u].w};
-#pragma unroll
-                    for (int k = 0; k < 4; k++) { if (dd[k] >= 0) wv[4 * u + k] = probe[dd[k] >> 5]; else wv[4 * u + k].bits = 0u; } }
-#pragma unroll
-                for (int u = 0; u < 4; u++) { const int dd[4] = {dv[u].x, dv[u].y, dv[u].z, dv[u].w};
-#pragma unroll
-                    for (int k = 0; k < 4; k++) if (dd[k] >= 0 && ((wv[4 * u + k].bits >> (dd[k] & 31)) & 1u)) put_hit(dd[k], wv[4 * u + k], a, (uint8_t)(tw[u] >> (8 * k))); }
-            }
-            done = pre + (n4 << 2);
-        }
-#endif
-        const int64_t NT4 = 4LL * NT;
-        for (int64_t i0 = done + c.tid(); i0 < len; i0 += NT4) {
-            int dd[4]; uint8_t tv[4]; S1Probe wv[4];
-            for (int u = 0; u < 4; u++) { int64_t i = i0 + (int64_t)u * NT; const bool in = i < len; dd[u] = in ? tm.docs[i] : -1; tv[u] = (in && tm.tf) ? tm.tf[i] : (uint8_t)1; }
-            for (int u = 0; u < 4; u++) { if (dd[u] >= 0) wv[u] = probe[dd[u] >> 5]; else wv[u].bits = 0u; }
-            for (int u = 0; u < 4; u++) if (dd[u] >= 0 && ((wv[u].bits >> (dd[u] & 31)) & 1u)) put_hit(dd[u], wv[u], a, tv[u]);
-        }
-    };
     if (forward) {
         // Batches of FW_G candidates per warp: their forward lists (a few dozen to a few hundred (term, tf) pairs each) are walked as ONE
         // concatenated range, so a lane has several independent loads in flight instead of one dependent chain per candidate. The
@@ -208,14 +166,95 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
                 }
             }
         }
-        for (int t = 0; t < T; t++) if (sh.order[t] >= 0 && sh.terms[t].term_id < 0) stream_term(sh.terms[t], sh.order[t]);      // LD1 unions have no term id
-    } else {
-        for (int t = 0; t < T; t++) if (sh.order[t] >= 0) stream_term(sh.terms[t], sh.order[t]);
+    }
+    // Streamed lists (every scored list in stream mode; in forward mode the LD1 unions, which have no term id), walked container-major:
+    // for every container that holds candidates, in ascending order, its 2048 bitset words go into shared memory with the candidates
+    // before each word (one block scan), the global words are zeroed, and then every streamed posting that falls into the container
+    // is tested against that window. Postings in containers without candidates are never loaded. A hit's slot is its rank inside the
+    // container, so it lands in the container's tf block (cpad) and sub-chunk without any per-shard table.
+    if (c.tid() == 0) { int n = 0; for (int t = 0; t < T; t++) if (sh.order[t] >= 0 && (!forward || sh.terms[t].term_id < 0)) sh.sterm[n++] = t; sh.bcast[3] = n; }
+    c.sync();
+    const int nS = sh.bcast[3];
+    if (nS > 0) {
+        // where every streamed list enters every container: the index's skip table for rows of >= 512 postings, otherwise (short rows,
+        // LD1 unions) one binary search per (list, container boundary), all of them in parallel before the walk
+        for (int i = c.tid(); i < (ncont + 1) * nS; i += NT) {
+            const int cc = i / nS; const TermS& tm = sh.terms[sh.sterm[i - cc * nS]];
+            ws.loff[i] = tm.skip ? tm.skip[cc] : (int32_t)lower_bound_i32(tm.docs, 0, tm.len, (int32_t)(cc << 16));
+        }
+        c.sync();
+        constexpr int LONG = 2048;                 // a (list, container) range this long is streamed on its own with 16-byte loads
+        const int per = CONT_WORDS / NT;           // window words per thread
+        struct alignas(16) W4 { unsigned v[4]; };
+        struct alignas(16) I4 { int32_t v[4]; };
+        for (int cc = 0; cc < ncont; cc++) {
+            const S1Cont ct = ctab[cc];
+            if (ct.cnt == 0) continue;
+            // the window (the bitset is allocated and zero up to whole containers, so the last one is read in full)
+            W4* gw = reinterpret_cast<W4*>(ws.bits + ((int64_t)cc << 11) + c.tid() * per); W4* sw = reinterpret_cast<W4*>(sh.win + c.tid() * per);
+            int mine = 0;
+            for (int k = 0; k < per / 4; k++) { const W4 x = gw[k]; sw[k] = x; mine += popc(x.v[0]) + popc(x.v[1]) + popc(x.v[2]) + popc(x.v[3]); }
+            { W4 z; z.v[0] = z.v[1] = z.v[2] = z.v[3] = 0u; for (int k = 0; k < per / 4; k++) gw[k] = z; }
+            int tot; int run = block_excl_scan(c, mine, sh.scan, tot);
+            for (int k = c.tid() * per; k < (c.tid() + 1) * per; k++) { sh.wrank[k] = (uint16_t)run; run += popc(sh.win[k]); }
+            if (c.warp() == 0) {      // the lists' ranges in this container; the short ones concatenated into one block-wide range
+                int carry = 0;
+                for (int s0 = 0; s0 < nS; s0 += WS) {
+                    const int s = s0 + c.lane(); int n = 0;
+                    if (s < nS) { const int lo = ws.loff[cc * nS + s], hi = ws.loff[(cc + 1) * nS + s]; sh.rlo[s] = lo; sh.rhi[s] = hi; n = hi - lo < LONG ? hi - lo : 0; }
+                    int incl = n;
+                    for (int d = 1; d < WS; d <<= 1) { int o = c.shfl(incl, c.lane() >= d ? c.lane() - d : 0); if (c.lane() >= d) incl += o; }
+                    if (s < nS) sh.rpre[s] = carry + incl - n;
+                    carry += c.shfl(incl, WS - 1);
+                }
+                if (c.lane() == 0) sh.rpre[nS] = carry;
+            }
+            c.sync();
+            auto put = [&](int d, uint8_t tfv, int a) {      // posting d of row a, inside this container
+                const int wl = (d >> 5) & (CONT_WORDS - 1); const unsigned wv = sh.win[wl], bit = 1u << (d & 31);
+                if (!(wv & bit)) return;
+                const int jc = sh.wrank[wl] + popc(wv & (bit - 1)), sub = jc / CHUNK; const int cnt_k = ct.cnt - sub * CHUNK < CHUNK ? ct.cnt - sub * CHUNK : CHUNK;
+                tfb[(int64_t)Ta * (ct.cpad + sub * CHUNK) + (int64_t)a * pad16(cnt_k) + (jc - sub * CHUNK)] = tfv;
+            };
+            {   // the short ranges: 8 postings per thread in flight; a thread's positions only grow, so its list cursor only moves forward
+                const int E = sh.rpre[nS]; int g = 0;
+                for (int e0 = c.tid(); e0 < E; e0 += 8 * NT) {
+                    int dd[8], ra[8]; uint8_t tv[8];
+#pragma unroll
+                    for (int u = 0; u < 8; u++) { const int e = e0 + u * NT; dd[u] = -1;
+                        if (e < E) { while (e >= sh.rpre[g + 1]) g++;
+                            const int t = sh.sterm[g]; const TermS& tm = sh.terms[t]; const int64_t i = sh.rlo[g] + (e - sh.rpre[g]);
+                            dd[u] = tm.docs[i]; tv[u] = tm.tf ? tm.tf[i] : (uint8_t)1; ra[u] = sh.order[t]; } }
+#pragma unroll
+                    for (int u = 0; u < 8; u++) if (dd[u] >= 0) put(dd[u], tv[u], ra[u]);
+                }
+            }
+            for (int s = 0; s < nS; s++) {      // the long ranges, one list at a time: 16 postings per thread in flight (four 16-byte id loads + four 4-byte tf loads)
+                const int lo = sh.rlo[s], len = sh.rhi[s] - lo; if (len < LONG) continue;
+                const TermS& tm = sh.terms[sh.sterm[s]]; const int a = sh.order[sh.sterm[s]];
+                const int32_t* docs = tm.docs + lo; const uint8_t* tfp = tm.tf ? tm.tf + lo : nullptr;
+                const int pre = (int)((0 - (reinterpret_cast<uintptr_t>(docs) >> 2)) & 3);
+                for (int i = c.tid(); i < pre; i += NT) put(docs[i], tfp ? tfp[i] : (uint8_t)1, a);
+                const I4* p4 = reinterpret_cast<const I4*>(docs + pre); const unsigned* t4 = tfp ? reinterpret_cast<const unsigned*>(tfp + pre) : nullptr;
+                const int n4 = (len - pre) >> 2;
+                for (int g0 = c.tid(); g0 < n4; g0 += 4 * NT) {
+                    I4 dv[4]; unsigned tw[4];
+#pragma unroll
+                    for (int u = 0; u < 4; u++) { const int g = g0 + u * NT; if (g < n4) { dv[u] = p4[g]; tw[u] = t4 ? t4[g] : 0x01010101u; } else { dv[u].v[0] = dv[u].v[1] = dv[u].v[2] = dv[u].v[3] = -1; tw[u] = 0u; } }
+#pragma unroll
+                    for (int u = 0; u < 4; u++)
+#pragma unroll
+                        for (int k = 0; k < 4; k++) if (dv[u].v[k] >= 0) put(dv[u].v[k], (uint8_t)(tw[u] >> (8 * k)), a);
+                }
+                for (int i = pre + (n4 << 2) + c.tid(); i < len; i += NT) put(docs[i], tfp ? tfp[i] : (uint8_t)1, a);
+            }
+            c.sync();      // the window is rewritten for the next container
+        }
     }
     c.sync();
     IFX_LTICK(3);   // tf lookups
     // ---- 4. bitset back to all-zero; record, queue, roofline accounting (SURVEY 8d)
-    clear_bits();
+    clear_bits(nS == 0);
     IFX_LTICK(4);   // bitset cleared
     if (c.tid() == 0) {
         rec.off_cand = a1; rec.off_dl = a1 + (((long long)n_cand * 4 + 31) & ~31LL); rec.off_chunk = a2; rec.off_terms = a2 + (long long)chunk_bytes; rec.off_tf = a2 + (long long)(chunk_bytes + term_bytes);
