@@ -5,7 +5,7 @@
 //     the hardware ones. This is the product.
 //   * IFX_EMU build (g++, tests only): Ctx == one host thread (group size 1, warp size 1). The kernels are host functions
 //     and the launch shim of ifx_api.inl calls them once per block, so the CPU test suite runs the product's host driver
-//     and kernels and checks them against the oracle without a GPU. It is never loaded by the product.
+//     and kernels, the index build's included, and checks them against the oracle without a GPU. It is never loaded by the product.
 #pragma once
 #include <stdint.h>
 #include <stddef.h>
@@ -155,6 +155,7 @@ struct Ctx {
 };
 inline unsigned atomic_or(unsigned* p, unsigned v) { unsigned o = *p; *p = o | v; return o; }
 inline int atomic_add(int* p, int v) { int o = *p; *p = o + v; return o; }
+inline unsigned atomic_add(unsigned* p, unsigned v) { unsigned o = *p; *p = o + v; return o; }
 inline unsigned atomic_and(unsigned* p, unsigned v) { unsigned o = *p; *p = o & v; return o; }
 inline int atomic_min(int* p, int v) { int o = *p; if (v < o) *p = v; return o; }
 inline int atomic_max(int* p, int v) { int o = *p; if (v > o) *p = v; return o; }
@@ -186,6 +187,7 @@ struct Ctx {
 };
 __device__ __forceinline__ unsigned atomic_or(unsigned* p, unsigned v) { return atomicOr(p, v); }
 __device__ __forceinline__ int atomic_add(int* p, int v) { return atomicAdd(p, v); }
+__device__ __forceinline__ unsigned atomic_add(unsigned* p, unsigned v) { return atomicAdd(p, v); }
 __device__ __forceinline__ unsigned atomic_and(unsigned* p, unsigned v) { return atomicAnd(p, v); }
 __device__ __forceinline__ int atomic_min(int* p, int v) { return atomicMin(p, v); }
 __device__ __forceinline__ int atomic_max(int* p, int v) { return atomicMax(p, v); }

@@ -115,18 +115,19 @@ IFX_FN void prepare_query(const DevIndex& ix, const uint16_t* text, int len, int
 
 // ---------------------------------------------------------------------------------------------------------------
 // block primitives
-struct ScanTmp { int w[33]; };
+template <class T> struct ScanTmpT { T w[33]; };
+using ScanTmp = ScanTmpT<int>;
 
-IFX_FN int block_excl_scan(const Ctx& c, int v, ScanTmp& tmp, int& total) {
+template <class T> IFX_FN T block_excl_scan(const Ctx& c, T v, ScanTmpT<T>& tmp, T& total) {
 #ifdef IFX_EMU
     (void)c; (void)tmp; total = v; return 0;
 #else
-    int incl = v;
-    for (int d = 1; d < 32; d <<= 1) { int o = __shfl_up_sync(0xffffffffu, incl, d); if (c.lane() >= d) incl += o; }
+    T incl = v;
+    for (int d = 1; d < 32; d <<= 1) { T o = __shfl_up_sync(0xffffffffu, incl, d); if (c.lane() >= d) incl += o; }
     if (c.lane() == 31) tmp.w[c.warp()] = incl;
     c.sync();
-    int base = 0, tot = 0, nw = c.nwarps();
-    for (int i = 0; i < nw; i++) { int x = tmp.w[i]; if (i < c.warp()) base += x; tot += x; }
+    T base = 0, tot = 0; int nw = c.nwarps();
+    for (int i = 0; i < nw; i++) { T x = tmp.w[i]; if (i < c.warp()) base += x; tot += x; }
     total = tot;
     c.sync();
     return base + incl - v;

@@ -1,6 +1,6 @@
 // TEST-ONLY host emulation of the infidex_b200 kernels (Ctx == one host thread). The product's host driver runs unchanged and
-// its launch shim calls the kernels as host functions, so the CPU test suite checks the launch sequence and the kernel logic
-// against the oracle without a GPU. Never loaded by the product package.
+// its launch shim calls the kernels as host functions, so the CPU test suite checks the launch sequence and the kernel logic,
+// from the device-side index build to the final results, against the oracle without a GPU. Never loaded by the product package.
 #define IFX_EMU 1
 #include "../../infidex_b200/csrc/ifx_api.inl"
 
