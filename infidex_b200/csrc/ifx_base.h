@@ -242,7 +242,8 @@ struct QueryPlan {
 };
 
 struct BatchCounters { int32_t n_fuzzy_items; int32_t overflow; unsigned long long fuzzy_pool_used; unsigned long long algo_bytes; unsigned long long s1_ns_sum; unsigned long long s1_ns_max; unsigned long long s1_cand_sum;
-                       unsigned long long s1_pool_used; int32_t s1_deferred, s1_n_light, s1_n_heavy, s1_wave, s1_n_mid, n_short; };
+                       unsigned long long s1_pool_used; int32_t s1_deferred, s1_n_light, s1_n_heavy, s1_wave, s1_n_mid, n_short;
+                       int32_t n_tf_pairs, n_tf_groups; };     // the wave's term-major tf lookups: TfPairs appended by stage1_lookup, distinct terms among them
 
 struct FuzzyItem { int32_t query; int32_t slot; };
 

@@ -186,7 +186,7 @@ struct S1Workspace {
     int32_t* loff;         // [n_cont + 1][streamed lists] offset of the first posting of each streamed list in container c (scratch of the tf lookups)
     int32_t* cstart;       // [n_cont + 1] candidates before container c
     int32_t* cfirst;       // [n_cont + 1] chunks before container c
-    int32_t* ctab;         // [n_cont] packed S1Cont records (16 bytes each) for the tf lookups
+    int32_t* cpad;         // [n_cont + 1] padded tf slots before container c
     int64_t cand_cap, buf_cap;
 };
 

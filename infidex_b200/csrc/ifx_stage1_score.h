@@ -16,13 +16,14 @@ namespace ifx {
 struct S1Chunk { int32_t start, cnt; int64_t tf_off; };                       // tf_off: bytes from the query's tf base
 struct S1TermP { float idf, max_score, suffix_after; int32_t pad; };
 struct S1Rec {
-    int64_t off_cand, off_dl, off_tf, off_chunk, off_terms;                    // byte offsets into the batch pool
+    int64_t off_cand, off_dl, off_tf, off_chunk, off_terms, off_ctab;          // byte offsets into the batch pool
     int32_t n_cand, n_chunks, n_terms, max_cnt;
     int32_t state;                                                            // 0 nothing to score, 1 light / 4 mid (score_warp), 3 heavy (score_cta), 2 deferred (pool full), -1 overflow
     int32_t K, path, pad;
 };
 struct S1Queues { int32_t* light; int32_t* mid; int32_t* heavy; };
-struct alignas(16) S1Cont { int32_t cstart, cnt, cpad, cfirst; };                // per container: candidates before it, its candidates, padded tf slots before it, chunks before it                           // query ids appended by stage1_lookup (counters in BatchCounters)
+struct alignas(16) S1Cont { int32_t cstart, cnt, cpad, cfirst; };                // per container: candidates before it, its candidates, padded tf slots before it, chunks before it
+struct TfPair { int32_t term, q, row; };      // a dictionary list whose tf bytes k_tf_terms fills: term id, query, row of the query's tf matrix
 
 IFX_FN int pad16(int x) { return (x + 15) & ~15; }
 constexpr int DEL_BIT = (int)0x80000000;
@@ -37,13 +38,14 @@ constexpr int W_K = 512;             // heap capacity kept in shared memory per 
 // ---------------------------------------------------------------------------------------------------------------
 // stage1_lookup: called right after stage1_select by the same CTA. Candidates are the bits of ws.bits.
 //   1. count + expand the bitset into the pool (ascending ids), candidates before every container
-//   2. document lengths, deleted flags, chunk table
-//   3. tf of every (term, candidate): either the posting lists streamed container by container against a shared-memory window of
-//      the candidate bitset (coalesced; only containers that hold candidates), or -- few candidates relative to the lists -- one
-//      forward-index read per candidate
+//   2. document lengths, deleted flags, chunk table, container table
+//   3. tf of every (term, candidate): either one forward-index read per candidate (few candidates relative to the lists), or the
+//      dictionary lists are left to k_tf_terms, which reads each distinct list once for all queries of the wave: one TfPair per list
+//      is appended to `pairs`. LD1 unions (this query's own lists) are streamed here, container by container against a shared-memory
+//      window of the candidate bitset (coalesced; only containers that hold candidates).
 //   4. bitset cleared again (in the container walk, or here when nothing was streamed)
 IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, int path, int q, S1Workspace& ws, S1LookupShared& sh, S1Rec* recs,
-                          unsigned char* spool, unsigned long long spool_cap, S1Queues queues, BatchCounters* bc, Stage1Out out, int fwd_avg_bytes, int force_mode) {
+                          unsigned char* spool, unsigned long long spool_cap, S1Queues queues, BatchCounters* bc, TfPair* pairs, Stage1Out out, int fwd_avg_bytes, int force_mode) {
     S1Rec& rec = recs[q]; const int NT = c.nthreads(), NW = c.nwarps(); constexpr int WS = Ctx::WS;
 #if !defined(IFX_EMU) && defined(IFX_S1_TIMERS)
     long long lmark = 0; if (c.tid() == 0) { asm volatile("mov.u64 %0, %%clock64;" : "=l"(lmark) :: "memory"); if (out.dbg) for (int k = 11; k < 18; k++) out.dbg[k] = 0; }
@@ -117,22 +119,23 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
         const int cc = c0 + c.tid(); const int cntc = cc < ncont ? ws.cstart[cc + 1] - ws.cstart[cc] : 0;
         const int nch = (cntc + CHUNK - 1) / CHUNK; const int slots = (cntc / CHUNK) * CHUNK + pad16(cntc % CHUNK);
         int t1, t2; const int e1 = block_excl_scan(c, nch, sh.scan, t1); const int e2 = block_excl_scan(c, slots, sh.scan, t2);
-        if (cc < ncont) { ws.cfirst[cc] = n_chunks + e1;
-                          S1Cont ct; ct.cstart = ws.cstart[cc]; ct.cnt = cntc; ct.cpad = n_slots + e2; ct.cfirst = n_chunks + e1; reinterpret_cast<S1Cont*>(ws.ctab)[cc] = ct; }
+        if (cc < ncont) { ws.cfirst[cc] = n_chunks + e1; ws.cpad[cc] = n_slots + e2; }
         if (cntc > 0) atomic_max(&sh.bcast[1], cntc < CHUNK ? cntc : CHUNK);
         n_chunks += t1; n_slots += t2;
     }
     c.sync();
-    const int max_cnt = sh.bcast[1]; const S1Cont* ctab = reinterpret_cast<const S1Cont*>(ws.ctab);
+    const int max_cnt = sh.bcast[1];
     const unsigned long long tf_bytes = (unsigned long long)(Ta > 0 ? Ta : 1) * (unsigned long long)n_slots;
-    const unsigned long long chunk_bytes = ((unsigned long long)n_chunks * sizeof(S1Chunk) + 15ULL) & ~15ULL, term_bytes = (unsigned long long)(Ta > 0 ? Ta : 1) * sizeof(S1TermP);
-    const long long a2 = pool_alloc(chunk_bytes + term_bytes + tf_bytes + 64);
+    const unsigned long long chunk_bytes = ((unsigned long long)n_chunks * sizeof(S1Chunk) + 15ULL) & ~15ULL, ctab_bytes = (unsigned long long)ncont * sizeof(S1Cont),
+                             term_bytes = (unsigned long long)(Ta > 0 ? Ta : 1) * sizeof(S1TermP);
+    const long long a2 = pool_alloc(chunk_bytes + ctab_bytes + term_bytes + tf_bytes + 64);
     if (a2 < 0) { give_up(a2); return; }
-    S1Chunk* chunks = reinterpret_cast<S1Chunk*>(spool + a2); S1TermP* tparams = reinterpret_cast<S1TermP*>(spool + a2 + chunk_bytes);
-    uint8_t* tfb = spool + a2 + chunk_bytes + term_bytes;
+    S1Chunk* chunks = reinterpret_cast<S1Chunk*>(spool + a2); S1Cont* ctab = reinterpret_cast<S1Cont*>(spool + a2 + chunk_bytes);
+    S1TermP* tparams = reinterpret_cast<S1TermP*>(spool + a2 + chunk_bytes + ctab_bytes); uint8_t* tfb = spool + a2 + chunk_bytes + ctab_bytes + term_bytes;
     for (int cc = c.tid(); cc < ncont; cc += NT) {
         const int cntc = ws.cstart[cc + 1] - ws.cstart[cc]; const int nch = (cntc + CHUNK - 1) / CHUNK;
-        for (int s = 0; s < nch; s++) { S1Chunk ch; ch.start = ws.cstart[cc] + s * CHUNK; ch.cnt = cntc - s * CHUNK < CHUNK ? cntc - s * CHUNK : CHUNK; ch.tf_off = (int64_t)Ta * (ctab[cc].cpad + s * CHUNK); chunks[ws.cfirst[cc] + s] = ch; }
+        S1Cont ct; ct.cstart = ws.cstart[cc]; ct.cnt = cntc; ct.cpad = ws.cpad[cc]; ct.cfirst = ws.cfirst[cc]; ctab[cc] = ct;
+        for (int s = 0; s < nch; s++) { S1Chunk ch; ch.start = ct.cstart + s * CHUNK; ch.cnt = cntc - s * CHUNK < CHUNK ? cntc - s * CHUNK : CHUNK; ch.tf_off = (int64_t)Ta * (ct.cpad + s * CHUNK); chunks[ct.cfirst + s] = ch; }
     }
     for (int t = c.tid(); t < T; t += NT) if (sh.order[t] >= 0) { S1TermP tp; tp.idf = sh.terms[t].idf; tp.max_score = sh.terms[t].max_score; tp.suffix_after = sh.terms[t].suffix_after; tp.pad = 0; tparams[sh.order[t]] = tp; }
     {   // zero the tf matrix (16-byte stores; the block is 16-byte aligned and padded)
@@ -167,12 +170,15 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
             }
         }
     }
-    // Streamed lists (every scored list in stream mode; in forward mode the LD1 unions, which have no term id), walked container-major:
-    // for every container that holds candidates, in ascending order, its 2048 bitset words go into shared memory with the candidates
-    // before each word (one block scan), the global words are zeroed, and then every streamed posting that falls into the container
-    // is tested against that window. Postings in containers without candidates are never loaded. A hit's slot is its rank inside the
-    // container, so it lands in the container's tf block (cpad) and sub-chunk without any per-shard table.
-    if (c.tid() == 0) { int n = 0; for (int t = 0; t < T; t++) if (sh.order[t] >= 0 && (!forward || sh.terms[t].term_id < 0)) sh.sterm[n++] = t; sh.bcast[3] = n; }
+    else {      // stream mode: the dictionary lists are read by k_tf_terms, once per wave for every query that scores them (in any order)
+        for (int t = c.tid(); t < T; t += NT) if (sh.order[t] >= 0 && sh.terms[t].term_id >= 0) { TfPair pr; pr.term = sh.terms[t].term_id; pr.q = q; pr.row = sh.order[t]; pairs[atomic_add(&bc->n_tf_pairs, 1)] = pr; }
+    }
+    // The LD1 unions (no term id: this query's own lists in the fuzzy pool), walked container-major: for every container that holds
+    // candidates, in ascending order, its 2048 bitset words go into shared memory with the candidates before each word (one block
+    // scan), the global words are zeroed, and then every streamed posting that falls into the container is tested against that window.
+    // Postings in containers without candidates are never loaded. A hit's slot is its rank inside the container, so it lands in the
+    // container's tf block (cpad) and sub-chunk without any per-shard table.
+    if (c.tid() == 0) { int n = 0; for (int t = 0; t < T; t++) if (sh.order[t] >= 0 && sh.terms[t].term_id < 0) sh.sterm[n++] = t; sh.bcast[3] = n; }
     c.sync();
     const int nS = sh.bcast[3];
     if (nS > 0) {
@@ -257,7 +263,8 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
     clear_bits(nS == 0);
     IFX_LTICK(4);   // bitset cleared
     if (c.tid() == 0) {
-        rec.off_cand = a1; rec.off_dl = a1 + (((long long)n_cand * 4 + 31) & ~31LL); rec.off_chunk = a2; rec.off_terms = a2 + (long long)chunk_bytes; rec.off_tf = a2 + (long long)(chunk_bytes + term_bytes);
+        rec.off_cand = a1; rec.off_dl = a1 + (((long long)n_cand * 4 + 31) & ~31LL); rec.off_chunk = a2; rec.off_ctab = a2 + (long long)chunk_bytes;
+        rec.off_terms = a2 + (long long)(chunk_bytes + ctab_bytes); rec.off_tf = a2 + (long long)(chunk_bytes + ctab_bytes + term_bytes);
         rec.n_cand = n_cand; rec.n_chunks = n_chunks; rec.n_terms = Ta; rec.max_cnt = max_cnt; rec.K = p.depth; rec.path = path;
         const bool warp_ok = Ta <= W_TERMS && p.depth <= W_K;
         if (Ta == 0) rec.state = 0;
@@ -275,6 +282,119 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
         if (out.dbg) { out.dbg[0] = n_cand; out.dbg[6] = forward ? 1 : 2; out.dbg[7] = n_chunks; out.dbg[8] = max_cnt; out.dbg[9] = Ta; }
     }
     c.sync();
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Term-major tf lookups of one staging-pool wave (k_tf_count, k_tf_scan, k_tf_fill, k_tf_terms). The queries of a batch share most of
+// their dictionary lists, so the TfPairs that stage1_lookup appended are grouped by term -- a counting sort over a dictionary-sized
+// count array, which k_tf_terms leaves zeroed again -- and every distinct list is read once. A work item is a run of containers of a
+// list with a skip table, or the whole group for a shorter row; every query of the group intersects the list with its candidates
+// there, and a hit writes the tf byte where stage1_lookup laid out the slot. Every byte is written exactly once, so the order in which groups, pairs and
+// items are processed does not change the result.
+struct TfGroups {
+    const TfPair* pairs; TfPair* sorted;      // as appended / grouped by term
+    int32_t* tcnt;                            // [dictionary] pairs per term, then the term's group (all zero between waves)
+    int32_t* gterm; int32_t* gptr; int32_t* gcur; int32_t* iptr;   // per group: term, first pair, fill cursor, first work item ([n_groups] = totals)
+};
+constexpr int TF_ROW = 512, TF_QCAP = 256, TF_CRANGE = 4;      // rows without a skip table are shorter than TF_ROW (SKIP_MIN); queries per metadata load; containers per work item
+struct TfQuery { const int32_t* cand; const S1Cont* ctab; uint8_t* tfb; int64_t n_cand; int32_t Ta, row; };
+struct TfShared {
+    unsigned bits[CONT_WORDS]; int32_t rank[CONT_WORDS];      // the list's postings in one container, the postings before every word
+    int32_t ids[TF_ROW]; uint8_t tf[TF_ROW];                 // a row without a skip table
+    TfQuery qm[TF_QCAP]; S1Cont ct[TF_QCAP]; ScanTmp scan; int bcast[8];
+};
+
+IFX_FN int64_t lower_bound_cand(const int32_t* a, int64_t lo, int64_t hi, int32_t target) {   // candidates carry DEL_BIT: compared without it
+    while (lo < hi) { int64_t mid = lo + ((hi - lo) >> 1); if ((a[mid] & ~DEL_BIT) < target) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+
+// one CTA: the groups' first pairs and first work items (exclusive scans); tcnt[term] becomes the term's group
+IFX_FN void tf_group_scan(const Ctx& c, const DevIndex& ix, TfGroups G, int n_groups, ScanTmp& tmp) {
+    int pbase = 0, ibase = 0;
+    for (int g0 = 0; g0 < n_groups; g0 += c.nthreads()) {
+        const int g = g0 + c.tid(); int np = 0, ni = 0;
+        if (g < n_groups) { const int t = G.gterm[g]; np = G.tcnt[t]; ni = ix.skip_id[t] >= 0 ? (ix.n_cont + TF_CRANGE - 1) / TF_CRANGE : 1; G.tcnt[t] = g; }
+        int tp, ti; const int ep = block_excl_scan(c, np, tmp, tp); const int ei = block_excl_scan(c, ni, tmp, ti);
+        if (g < n_groups) { G.gptr[g] = G.gcur[g] = pbase + ep; G.iptr[g] = ibase + ei; }
+        pbase += tp; ibase += ti;
+    }
+    if (c.tid() == 0) { G.gptr[n_groups] = pbase; G.iptr[n_groups] = ibase; }
+}
+
+// Work item `it`: TF_CRANGE containers of a list with a skip table, or a whole shorter row. What the group's queries need (candidate
+// array, container table, tf matrix, row) is read into shared memory once per item, TF_QCAP queries at a time. In a container, the
+// list's postings become a bitmap of the container's 65 536 documents with the postings before every word, so each candidate of each
+// query is one bit test and, on a hit, one rank: no search, and the work is the queries' candidates in the container. A shorter row
+// (< 512 postings) sits in shared memory whole; each query searches the shorter of (its candidates, the row) in the longer. One warp
+// per query, or -- fewer queries than warps -- the whole CTA on one query after the other.
+IFX_FN void tf_terms_item(const Ctx& c, const DevIndex& ix, const TfGroups& G, int n_groups, int it, const S1Rec* recs, unsigned char* spool, TfShared& sh) {
+    const int NT = c.nthreads(), NW = c.nwarps();
+    if (c.warp() == 0) { const int g = (int)warp_lower_bound(c, G.iptr, 0, n_groups + 1, it + 1) - 1; if (c.lane() == 0) { sh.bcast[0] = g; sh.bcast[1] = 0; } }
+    c.sync();
+    const int g = sh.bcast[0]; const int term = G.gterm[g]; const int j0 = G.gptr[g], j1 = G.gptr[g + 1];
+    const int64_t r0 = ix.row_ptr[term], len = ix.row_ptr[term + 1] - r0; const int32_t* docs = ix.post_doc + r0; const uint8_t* tfs = ix.post_tf + r0;
+    const int sk = ix.skip_id[term];      // sk >= 0: containers [c0, c1) of the list; otherwise the whole row
+    const int32_t* skip = sk >= 0 ? ix.skip_ptr + (size_t)sk * (ix.n_cont + 1) : nullptr;
+    const int c0 = sk >= 0 ? (it - G.iptr[g]) * TF_CRANGE : 0, c1 = sk >= 0 ? (c0 + TF_CRANGE < ix.n_cont ? c0 + TF_CRANGE : ix.n_cont) : 0;
+    if (sk < 0) { for (int i = c.tid(); i < len; i += NT) { sh.ids[i] = docs[i]; sh.tf[i] = tfs[i]; } }      // len < TF_ROW (rows without a skip table)
+    for (int q0 = j0; q0 < j1; q0 += TF_QCAP) {
+        const int nq = j1 - q0 < TF_QCAP ? j1 - q0 : TF_QCAP;
+        for (int k = c.tid(); k < nq; k += NT) {
+            const TfPair pr = G.sorted[q0 + k]; const S1Rec& rc = recs[pr.q]; TfQuery m;
+            m.cand = reinterpret_cast<const int32_t*>(spool + rc.off_cand); m.ctab = reinterpret_cast<const S1Cont*>(spool + rc.off_ctab); m.tfb = spool + rc.off_tf;
+            m.n_cand = rc.n_cand; m.Ta = rc.n_terms; m.row = pr.row; sh.qm[k] = m;
+        }
+        c.sync();
+        const bool wide = nq < NW; const int kfirst = wide ? 0 : c.warp(), kstep = wide ? 1 : NW, e0 = wide ? c.tid() : c.lane(), estep = wide ? NT : Ctx::WS;
+        auto put = [&](const TfQuery& m, int64_t i, const S1Cont& ct, uint8_t v) {      // candidate i of the query (in container ct) has tf v
+            const int jc = (int)(i - ct.cstart), sub = jc / CHUNK; const int cnt_k = ct.cnt - sub * CHUNK < CHUNK ? ct.cnt - sub * CHUNK : CHUNK;
+            m.tfb[(int64_t)m.Ta * (ct.cpad + sub * CHUNK) + (int64_t)m.row * pad16(cnt_k) + (jc - sub * CHUNK)] = v;
+        };
+        if (sk < 0) {
+            const int n = (int)len;
+            for (int k = kfirst; k < nq; k += kstep) {
+                const TfQuery& m = sh.qm[k]; const int32_t* cand = m.cand;
+                if (m.n_cand <= n) {      // each candidate searched in the row
+                    for (int64_t i = e0; i < m.n_cand; i += estep) {
+                        const int d = cand[i] & ~DEL_BIT; const int p = (int)lower_bound_i32(sh.ids, 0, n, d);
+                        if (p < n && sh.ids[p] == d) put(m, i, m.ctab[d >> 16], sh.tf[p]);
+                    }
+                } else {                  // each posting searched among the candidates of its container
+                    for (int p = e0; p < n; p += estep) {
+                        const int d = sh.ids[p]; const S1Cont ct = m.ctab[d >> 16];
+                        const int64_t i = lower_bound_cand(cand, ct.cstart, ct.cstart + ct.cnt, d);
+                        if (i < ct.cstart + ct.cnt && (cand[i] & ~DEL_BIT) == d) put(m, i, ct, sh.tf[p]);
+                    }
+                }
+            }
+        }
+        for (int cc = c0; cc < c1; cc++) {
+            const int64_t lo = skip[cc], hi = skip[cc + 1];
+            if (lo == hi) continue;
+            const int stamp = (q0 - j0) / TF_QCAP * (ix.n_cont + 1) + cc + 1;      // unique within the item: no reset, no extra barrier
+            for (int k = c.tid(); k < nq; k += NT) { const S1Cont ct = sh.qm[k].ctab[cc]; sh.ct[k] = ct; if (ct.cnt > 0) sh.bcast[1] = stamp; }
+            for (int w = c.tid(); w < CONT_WORDS; w += NT) sh.bits[w] = 0u;
+            c.sync();
+            if (sh.bcast[1] != stamp) continue;      // no query of the group has candidates in the container
+            for (int64_t i = lo + c.tid(); i < hi; i += NT) { const int d = docs[i]; atomic_or(&sh.bits[(d >> 5) & (CONT_WORDS - 1)], 1u << (d & 31)); }
+            c.sync();
+            {   const int per = CONT_WORDS / NT; int mine = 0;
+                for (int w = c.tid() * per; w < (c.tid() + 1) * per; w++) mine += popc(sh.bits[w]);
+                int tot; int run = block_excl_scan(c, mine, sh.scan, tot);
+                for (int w = c.tid() * per; w < (c.tid() + 1) * per; w++) { sh.rank[w] = run; run += popc(sh.bits[w]); } }
+            c.sync();
+            for (int k = kfirst; k < nq; k += kstep) {
+                const TfQuery& m = sh.qm[k]; const S1Cont ct = sh.ct[k];
+                for (int64_t i = ct.cstart + e0; i < ct.cstart + ct.cnt; i += estep) {
+                    const int d = m.cand[i] & ~DEL_BIT; const int w = (d >> 5) & (CONT_WORDS - 1); const unsigned bit = 1u << (d & 31), wv = sh.bits[w];
+                    if (wv & bit) put(m, i, ct, tfs[lo + sh.rank[w] + popc(wv & (bit - 1))]);
+                }
+            }
+            c.sync();      // the bitmap and sh.ct are rewritten next
+        }
+        c.sync();      // sh.qm is rewritten next
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------

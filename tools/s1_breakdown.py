@@ -25,6 +25,17 @@ for i in order[:8]: print("%-36s cand=%7d T=%3d path=%d mode=%d chunks=%4d maxcn
 order = np.argsort(-k2)
 for i in order[:5]: print("K2 top: %-30s cand=%7d T=%3d chunks=%4d maxcnt=%4d light=%d K2=%.2f ms" % (qs[i][:30], nc[i], ta[i], nch[i], mx[i], light[i], k2[i]))
 
+# List sharing of the streamed tf lookups: every (query, dictionary list) pair of a stream-mode query reads 5 B per posting when
+# each query streams its own lists; read once per distinct list, the batch moves only the distinct lists' bytes.
+tt = np.zeros((NQ, 128, 3), np.int32); e._gpu.ifx_debug_stage1_terms(h, tt.ctypes.data_as(C.c_void_p))
+sel = ((mode == 2) & (nc > 0))[:, None] & (tt[:, :, 0] >= 0) & (tt[:, :, 2] != 0)
+ids, lens = tt[:, :, 0][sel], tt[:, :, 1][sel].astype(np.int64)
+if ids.size:
+    uniq, first = np.unique(ids, return_index=True)
+    per_q, distinct = 5 * lens.sum(), 5 * lens[first].sum()
+    print("streamed dictionary lists: %d (query, list) pairs over %d distinct lists (%.1f queries per list); bytes %.2f GB per query -> %.2f GB "
+          "distinct: byte-weighted sharing %.1fx (%d wave(s))" % (ids.size, uniq.size, ids.size / uniq.size, per_q / 1e9, distinct / 1e9, per_q / distinct, st.as_dict().get("s1_waves", 1)))
+
 if dbg[:, 11:16].sum() > 0:
     for name, sel in (("forward", mode == 1), ("stream", mode == 2)):
         if sel.any(): print(name, "lookup phases, mean kcycles [count+expand, lengths, chunk table+zero, tf lookups, clear]:", (dbg[sel, 11:16].mean(0) / 1e3).astype(int), "| selection sticks [sort, tier0/unions, tier1, -]:", (dbg[sel, 20:24].mean(0) / 1e3).astype(int))
