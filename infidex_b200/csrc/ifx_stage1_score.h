@@ -78,7 +78,8 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
         c.sync(); long long r = sh.bcast64[2]; c.sync(); return r;
     };
     auto give_up = [&](long long why) { clear_bits(true); if (c.tid() == 0) { rec.state = why == -2 ? -1 : 2; rec.n_cand = n_cand; rec.K = p.depth; rec.path = path; if (why != -2) atomic_add(&bc->s1_deferred, 1); else out.n[0] = -1; } c.sync(); };      // a query larger than the whole pool is an overflow, like every other fixed buffer
-    const long long a1 = pool_alloc(8ULL * (unsigned long long)n_cand + 64);
+    const unsigned long long a1_bytes = 8ULL * (unsigned long long)n_cand + 64;
+    const long long a1 = pool_alloc(a1_bytes);
     if (a1 < 0) { give_up(a1); return; }
     int32_t* cand = reinterpret_cast<int32_t*>(spool + a1); float* dlp = reinterpret_cast<float*>(spool + a1 + (((long long)n_cand * 4 + 31) & ~31LL));
     // ---- 1b. expand + candidates before every container
@@ -128,7 +129,10 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
     const unsigned long long tf_bytes = (unsigned long long)(Ta > 0 ? Ta : 1) * (unsigned long long)n_slots;
     const unsigned long long chunk_bytes = ((unsigned long long)n_chunks * sizeof(S1Chunk) + 15ULL) & ~15ULL, ctab_bytes = (unsigned long long)ncont * sizeof(S1Cont),
                              term_bytes = (unsigned long long)(Ta > 0 ? Ta : 1) * sizeof(S1TermP);
-    const long long a2 = pool_alloc(chunk_bytes + ctab_bytes + term_bytes + tf_bytes + 64);
+    const unsigned long long a2_bytes = chunk_bytes + ctab_bytes + term_bytes + tf_bytes + 64;
+    // both allocations live until the wave ends: when they do not fit the pool together, not even a wave that starts empty can hold
+    // the query, so it is an overflow like a single allocation larger than the pool (deferring it would repeat it in every wave)
+    const long long a2 = ((a1_bytes + 255ULL) & ~255ULL) + ((a2_bytes + 255ULL) & ~255ULL) > spool_cap ? -2 : pool_alloc(a2_bytes);
     if (a2 < 0) { give_up(a2); return; }
     S1Chunk* chunks = reinterpret_cast<S1Chunk*>(spool + a2); S1Cont* ctab = reinterpret_cast<S1Cont*>(spool + a2 + chunk_bytes);
     S1TermP* tparams = reinterpret_cast<S1TermP*>(spool + a2 + chunk_bytes + ctab_bytes); uint8_t* tfb = spool + a2 + chunk_bytes + ctab_bytes + term_bytes;

@@ -24,8 +24,8 @@ def build_pair(keys, schema, cols, gpu_lib=None):
     return eng, orc
 
 
-def compare_stage1(eng, orc, queries, depth=500):
-    keys, scores, n, status = eng.Stage1Batch(queries, depth)
+def compare_stage1(eng, orc, queries, depth=500, stats=None):
+    keys, scores, n, status = eng.Stage1Batch(queries, depth, stats)
     bad = []
     for i, q in enumerate(queries):
         r = orc.stage1(q, depth)
