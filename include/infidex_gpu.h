@@ -103,6 +103,14 @@ typedef struct ifx_index_image {
     const int32_t* prefix_global_card;/* [prefix.keys.n] DocSet cardinality over all shards (the selector's prefix rules are global) */
     int32_t shard_index, n_shards;
     int64_t doc_base;                 /* global internal id of this shard's document 0 */
+    /* SynonymMap (Synonyms/SynonymMap.cs): zero / NULL = no map, or a map without mappings (HasCanonicalMappings false). Otherwise one
+     * entry per key of the map's union-find (_parent): syn_keys[i] is the key (lower case, keys unique under OrdinalIgnoreCase) and
+     * syn_canon[i] = GetCanonical(key), non-empty. The device derives the coverage text CanonicalizeText(Normalize(IndexedText)) from
+     * text_chars with it. The rest of the image must have been built with the same map (the index text, metadata and prefix index are
+     * canonicalised; WordMatcher and the word idf are not), and ifx_query.text must be canonicalised with it too: an index is re-created
+     * whenever the map changes. */
+    ifx_strings syn_keys;
+    ifx_strings syn_canon;
 } ifx_index_image;
 
 typedef struct ifx_params {           /* ConfigurationParameters[400] + CoverageSetup defaults when zero-initialised via ifx_params_default */
@@ -113,7 +121,9 @@ typedef struct ifx_params {           /* ConfigurationParameters[400] + Coverage
 } ifx_params;
 
 typedef struct ifx_query {
-    const uint16_t* text;             /* after Trim + TextNormalizer.Normalize + ToLowerInvariant (SearchEngine.cs:264-274) */
+    const uint16_t* text;             /* after Trim + TextNormalizer.Normalize + ToLowerInvariant (SearchEngine.cs:264-274); with a SynonymMap
+                                       * (image syn_keys.n > 0) then SynonymMap.CanonicalizeText and TextNormalizer.Normalize once more
+                                       * (SearchPipeline.Execute), i.e. the text the pipeline works on */
     int32_t len;
     int32_t max_results;              /* Query.MaxNumberOfRecordsToReturn */
     int32_t coverage_depth;           /* Query.CoverageDepth (<= 1024) */

@@ -34,6 +34,14 @@ int ifx_builder_set_global_lengths(ifx_builder* b, int n_shards, const float* co
 /* SearchEngine.Search step 1 (src/Infidex/SearchEngine.cs:264-274): Trim + TextNormalizer.Normalize + ToLowerInvariant. Returns the output length. */
 int ifx_host_prepare_query(const uint16_t* in, int n, uint16_t* out, int cap);
 
+/* SynonymMap of the engine (SearchEngine(..., synonymMap), Synonyms/SynonymMap.cs): the table (key, GetCanonical(key)) over every key of the
+ * map's union-find. Only before the first ifx_builder_add_docs; keys must be unique under OrdinalIgnoreCase, canonical strings non-empty
+ * (IFX_ERR_INVALID otherwise). An empty table is no map. The image carries the table (ifx_index_image.syn_keys / syn_canon). */
+int ifx_builder_set_synonyms(ifx_builder* b, const ifx_strings* keys, const ifx_strings* canon);
+/* The query text ifx_query.text expects from this builder's engine: ifx_host_prepare_query, then with a map CanonicalizeText and
+ * TextNormalizer.Normalize again (SearchEngine.cs:264-288, SearchPipeline.cs:68-71). Returns the output length, which may exceed n. */
+int ifx_builder_prepare_query(ifx_builder* b, const uint16_t* in, int n, uint16_t* out, int cap);
+
 /* filter / facet columns of the finished image (index = ifx_batch_result.facet_column) */
 int ifx_builder_num_columns(ifx_builder* b);
 int ifx_builder_column_name(ifx_builder* b, int c, uint16_t* buf, int cap);

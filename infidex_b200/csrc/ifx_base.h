@@ -104,6 +104,9 @@ struct DevIndex {
     // short-query path (ifx_short.h): champion lists of the 1-character prefixes, raw IndexedText of the documents that normalisation changed
     int32_t n_champ; const uint16_t* champ_chars; const int32_t* champ_off; const int32_t* champ_doc; const float* champ_score;
     int32_t n_raw; const int32_t* raw_doc; const int64_t* raw_off; const uint16_t* raw_chars;
+    // the document text of the coverage stage: CanonicalizeText(Normalize(IndexedText)) with a SynonymMap (derived at index creation,
+    // ifx_build.h k_canon_*), else the same pointers as text / text_off
+    const uint16_t* cov_text; const int64_t* cov_text_off;
 };
 
 IFX_FN uint64_t hash64(const uint16_t* s, int n) {

@@ -93,4 +93,45 @@ IFX_GLOBAL void IFX_BOUNDS(512) k_bitmap_rank(int bm_words, const unsigned* bm_b
     }
 }
 
+// ---- coverage text of an index with a SynonymMap: SynonymMap.CanonicalizeText(Normalize(IndexedText)) per document, one thread each --
+// (SearchPipeline.cs:470-489 canonicalises it again for every (query, candidate) pair; it is a pure function of the document text.)
+// keys: the map's keys folded through `upper` (StringComparer.OrdinalIgnoreCase), hashed; canon[i]: GetCanonical of key i.
+struct SynDev { StrDict keys; const uint16_t* canon_chars; const uint32_t* canon_off; };
+
+// Returns the canonical text's length; `out` may be null (count pass). Delimiters are copied; every maximal run of non-delimiters is
+// trimmed (char.IsWhiteSpace), dropped when nothing is left, lower-cased (ToLowerInvariant) and replaced by its root when the map has it.
+IFX_FN int64_t canon_emit(const DevIndex& ix, const SynDev& s, int doc, uint16_t* out) {
+    const int64_t t0 = ix.text_off[doc], t1 = ix.text_off[doc + 1]; const uint16_t* t = ix.text;
+    int64_t o = 0;
+    for (int64_t i = t0; i < t1;) {
+        if (ix.cflags[t[i]] & 4) { if (out) out[o] = t[i]; o++; i++; continue; }
+        int64_t b = i; while (i < t1 && !(ix.cflags[t[i]] & 4)) i++;
+        int64_t e = i; while (b < e && (ix.cflags[t[b]] & 2)) b++; while (e > b && (ix.cflags[t[e - 1]] & 2)) e--;
+        if (b == e) continue;
+        const int n = (int)(e - b); int k = -1;
+        if (s.keys.n > 0 && e - b < 0x7fffffff) {                      // dict_lookup over the folded token, folded on the fly
+            uint64_t h = 0xcbf29ce484222325ULL ^ (uint64_t)n;
+            for (int64_t j = b; j < e; j++) { h ^= ix.upper[ix.lower[t[j]]]; h *= 0x100000001b3ULL; }
+            h ^= h >> 29; h *= 0xbf58476d1ce4e5b9ULL; h ^= h >> 32; h |= 1ULL;
+            for (uint32_t slot = (uint32_t)(h >> 7) & s.keys.hmask;; slot = (slot + 1) & s.keys.hmask) {
+                const uint64_t hk = s.keys.hkeys[slot]; if (hk == 0) break;
+                if (hk != h) continue;
+                const int idx = s.keys.hvals[slot]; const uint32_t kb = s.keys.off[idx];
+                if ((int)(s.keys.off[idx + 1] - kb) != n) continue;
+                bool eq = true; for (int j = 0; j < n; j++) if (s.keys.chars[kb + j] != ix.upper[ix.lower[t[b + j]]]) { eq = false; break; }
+                if (eq) { k = idx; break; }
+            }
+        }
+        if (k >= 0) { const uint32_t cb = s.canon_off[k], ce = s.canon_off[k + 1]; if (out) for (uint32_t j = cb; j < ce; j++) out[o + (j - cb)] = s.canon_chars[j]; o += ce - cb; }
+        else { if (out) for (int64_t j = b; j < e; j++) out[o + (j - b)] = ix.lower[t[j]]; o += n; }
+    }
+    return o;
+}
+IFX_GLOBAL void IFX_BOUNDS(256) k_canon_count(DevIndex ix, SynDev s, unsigned* cnt) {
+    Ctx c; const int d = c.block() * c.nthreads() + c.tid(); if (d < ix.n_docs) cnt[d] = (unsigned)canon_emit(ix, s, d, nullptr);
+}
+IFX_GLOBAL void IFX_BOUNDS(256) k_canon_fill(DevIndex ix, SynDev s, const int64_t* off, uint16_t* out) {
+    Ctx c; const int d = c.block() * c.nthreads() + c.tid(); if (d < ix.n_docs) canon_emit(ix, s, d, out + off[d]);
+}
+
 }  // namespace ifx

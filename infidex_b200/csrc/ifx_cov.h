@@ -179,7 +179,7 @@ IFX_FN void prepare_cov_query(const DevIndex& ix, const uint16_t* q, int qlen, C
 //   [2 + fd .. 2 + fd + dc)  tokens of >= 2 units, first occurrence only (case-insensitive), in document order
 // Returns the number of words; `out` may be null (count pass).
 IFX_FN int doc_tokens_emit(const DevIndex& ix, int doc, uint32_t* out) {
-    const int64_t t0 = ix.text_off[doc]; const Str d{ix.text + t0, (int)(ix.text_off[doc + 1] - t0)};
+    const int64_t t0 = ix.cov_text_off[doc]; const Str d{ix.cov_text + t0, (int)(ix.cov_text_off[doc + 1] - t0)};
     Tok dt[MAX_DTOK]; bool ovf = false; int draw = 0, dc = 0, fd = 0; unsigned tok_or = 0;
     int i = 0; const int maxtok = d.n / 2 + 1;
     while (i < d.n) {
@@ -210,7 +210,7 @@ struct CovResult { float score; float score0; uint8_t tie; int word_hits; int ov
 IFX_FN CovResult coverage_fusion(const DevIndex& ix, const CovQuery& c, const uint16_t* qtext, int doc, int lcs, float bm25) {
     CovResult R; R.score = 0.f; R.score0 = 0.f; R.tie = 0; R.word_hits = 0; R.overflow = 0;
     const Str q{qtext, c.qlen};
-    const int64_t t0 = ix.text_off[doc]; const Str d{ix.text + t0, (int)(ix.text_off[doc + 1] - t0)};
+    const int64_t t0 = ix.cov_text_off[doc]; const Str d{ix.cov_text + t0, (int)(ix.cov_text_off[doc + 1] - t0)};
     const int qc = c.n_tok;
     // ---- doc tokens from the index's token table: every token (fdt), and the deduplicated tokens of >= 2 units (dt)
     const uint32_t* tt = ix.tok_tab + ix.tok_ptr[doc];

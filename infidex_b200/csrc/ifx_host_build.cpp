@@ -26,6 +26,7 @@
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
+#include <unordered_map>
 
 namespace {
 #include "chartables.inc"
@@ -83,6 +84,28 @@ template <class T, class Cmp> struct DotnetIntroSort {
     void sort(T* k, int n) { if (n < 2) return; int lg = 0; for (unsigned v = (unsigned)n; v >>= 1;) lg++; intro(k, n, 2 * (lg + 1)); }
 };
 inline bool is_ws(char16_t c) { static std::vector<uint8_t> ws = [] { std::vector<uint8_t> w(65536, 0); for (int i = 0; i < IFX_SPACE_LIST_N; i++) w[IFX_SPACE_LIST[i]] = 1; return w; }(); return ws[c] != 0; }
+
+// SynonymMap table: key folded as StringComparer.OrdinalIgnoreCase folds it (upper-invariant per UTF-16 unit) -> GetCanonical(key)
+struct SynTable {
+    std::vector<uint16_t> upper;
+    struct H { size_t operator()(const str& s) const { return std::hash<sv>()(sv(s)); } };
+    std::unordered_map<str, str, H> canon;
+    SynTable() : upper(65536) { for (int i = 0; i < 65536; i++) upper[i] = (uint16_t)i; for (int i = 0; i < IFX_UPPER_PAIRS_N; i++) upper[IFX_UPPER_PAIRS[i][0]] = IFX_UPPER_PAIRS[i][1]; }
+    str fold(sv s) const { str r(s); for (auto& c : r) c = (char16_t)upper[c]; return r; }
+};
+// SynonymMap.CanonicalizeText (SynonymMap.cs:153-186): delimiters copied; every maximal run of non-delimiters -> GetCanonical(run):
+// "" when blank, else the trimmed, lower-cased run replaced by its root when the map has it
+void canon_into(sv in, str& out, const SynTable& S) {
+    out.clear(); str tok;
+    for (size_t i = 0; i < in.size();) {
+        if (is_delim(in[i])) { out.push_back(in[i++]); continue; }
+        size_t s = i; while (i < in.size() && !is_delim(in[i])) i++;
+        size_t b = s, e = i; while (b < e && is_ws(in[b])) b++; while (e > b && is_ws(in[e - 1])) e--;
+        if (b == e) continue;
+        tok.assign(in.substr(b, e - b)); lower_inplace(tok);
+        auto it = S.canon.find(S.fold(tok)); out += it == S.canon.end() ? tok : it->second;
+    }
+}
 
 // string interner: open addressing over a char arena; ids in first-insertion order
 struct Interner {
@@ -206,6 +229,9 @@ struct ifx_builder {
     std::vector<int32_t> raw_doc; std::vector<char16_t> raw_chars; std::vector<int64_t> raw_off;
     std::vector<ifx_column> cols; std::vector<std::vector<int32_t>> col_ids; std::vector<std::vector<char16_t>> col_chars; std::vector<std::vector<uint32_t>> col_off; std::vector<str> col_names;
     std::vector<int> col_kind;                                         // kind of the column's field
+    // SynonymMap (ifx_builder_set_synonyms): empty = no map
+    SynTable syn; std::vector<char16_t> syn_key_chars, syn_canon_chars; std::vector<uint32_t> syn_key_off{0}, syn_canon_off{0};
+    bool has_syn() const { return !syn.canon.empty(); }
 };
 
 static float compute_idf_host(int total, int df) {   // Bm25Scorer.ComputeIdf
@@ -223,6 +249,21 @@ ifx_builder* ifx_builder_create(int nfields, const uint16_t* names, const int32_
     return b;
 }
 void ifx_builder_destroy(ifx_builder* b);
+
+int ifx_builder_set_synonyms(ifx_builder* b, const ifx_strings* keys, const ifx_strings* canon) {
+    if (!b || !keys || !canon || b->finished || !b->keys.empty()) return IFX_ERR_INVALID;
+    if (keys->n < 0 || keys->n != canon->n || (keys->n > 0 && (!keys->chars || !keys->off || !canon->chars || !canon->off))) return IFX_ERR_INVALID;
+    SynTable t; std::vector<char16_t> kc, cc; std::vector<uint32_t> ko{0}, co{0};
+    for (int i = 0; i < keys->n; i++) {
+        if (keys->off[i + 1] < keys->off[i] || canon->off[i + 1] <= canon->off[i]) return IFX_ERR_INVALID;   // canonical strings are never empty
+        sv k((const char16_t*)keys->chars + keys->off[i], keys->off[i + 1] - keys->off[i]), c((const char16_t*)canon->chars + canon->off[i], canon->off[i + 1] - canon->off[i]);
+        if (!t.canon.emplace(t.fold(k), str(c)).second) return IFX_ERR_INVALID;                                // two keys of one OrdinalIgnoreCase class
+        kc.insert(kc.end(), k.begin(), k.end()); ko.push_back((uint32_t)kc.size()); cc.insert(cc.end(), c.begin(), c.end()); co.push_back((uint32_t)cc.size());
+    }
+    if (kc.empty()) kc.push_back(0); if (cc.empty()) cc.push_back(0);
+    b->syn.canon.swap(t.canon); b->syn_key_chars.swap(kc); b->syn_canon_chars.swap(cc); b->syn_key_off.swap(ko); b->syn_canon_off.swap(co);
+    return IFX_OK;
+}
 
 int ifx_builder_add_docs(ifx_builder* b, int n, const int64_t* keys, const int32_t* kinds, const void* const* cols, const long long* const* offs) {
     if (b->finished) return IFX_ERR_INVALID;
@@ -250,22 +291,26 @@ int ifx_builder_finish(ifx_builder* b, int threads) {
         std::vector<int32_t> raw_doc; std::vector<char16_t> raw_chars; std::vector<int64_t> raw_len;   // documents whose raw IndexedText differs from its normalised form
     };
     std::vector<Part> parts(threads);
+    const bool syn = b->has_syn();
     auto work = [&](int t) {
         Part& P = parts[t]; P.terms.reset(new KeyedRecords(true)); P.prefix.reset(new KeyedRecords(false)); P.exact.reset(new KeyedRecords(false)); P.ld1.reset(new KeyedRecords(false));
         int d0 = (int)((int64_t)N * t / threads), d1 = (int)((int64_t)N * (t + 1) / threads);
-        str raw, nrm, idx, padded, wm, tmp; std::vector<std::pair<int, int>> bounds; std::vector<int> seen_words; std::vector<sv> tok_scratch;
+        str raw, nrm, idx, padded, wm, tmp, meta, ngr; std::vector<std::pair<int, int>> bounds; std::vector<int> seen_words; std::vector<sv> tok_scratch;
         for (int d = d0; d < d1; d++) {
             raw.clear(); bounds.clear();
             for (size_t k = 0; k < order.size(); k++) { bounds.emplace_back((int)(uint16_t)raw.size(), b->schema[order[k]].weight); raw += b->values[order[k]][d]; if (k + 1 < order.size()) raw.push_back(u'§'); }
             normalize_into(raw, nrm);                       // normalize(IndexedText): coverage doc text
             P.text.insert(P.text.end(), nrm.begin(), nrm.end()); P.text_len.push_back((int64_t)nrm.size());
-            idx = nrm; lower_inplace(idx);                  // VectorModel.IndexDocument: Normalize then ToLowerInvariant
-            // 3-grams of PAD PAD + text, then words (len >= 3)
-            padded.assign(2, (char16_t)0xFFFF); padded += idx;
+            idx = nrm; lower_inplace(idx);                  // VectorModel.IndexDocument: Normalize then ToLowerInvariant (then CanonicalizeText)
+            if (syn) { canon_into(idx, meta, b->syn); idx.swap(meta); normalize_into(idx, ngr); }
+            // 3-grams of PAD PAD + text, then words (len >= 3), over the text Tokenizer.EnumerateTokensForIndexing normalises once more
+            // (Tokenizer.cs:94-97: idempotent without a map; with one it collapses emptied tokens and maps the canonical forms' characters)
+            const str& tk = syn ? ngr : idx;
+            padded.assign(2, (char16_t)0xFFFF); padded += tk;
             auto fw_at = [&](int pos) { if (bounds.empty()) return 1.0f; int wi = 0; for (auto& bd : bounds) { if (bd.first <= pos) wi = bd.second; else break; } return wi < 3 ? b->field_weights[wi] : 1.0f; };
             if (padded.size() >= 3) for (size_t i = 0; i + 3 <= padded.size(); i++) { sv g(padded.data() + i, 3); if (g[0] == 0xFFFF && g[1] == 0xFFFF && g[2] == 0xFFFF) continue; P.terms->add_weighted(P.terms->key(g), d, fw_at((int)i)); }
-            for (size_t i = 0; i < idx.size();) { while (i < idx.size() && is_delim(idx[i])) i++; if (i >= idx.size()) break; size_t s = i; while (i < idx.size() && !is_delim(idx[i])) i++;
-                if (i - s >= 3) P.terms->add_weighted(P.terms->key(sv(idx.data() + s, i - s)), d, fw_at(2 + (int)s)); }
+            for (size_t i = 0; i < tk.size();) { while (i < tk.size() && is_delim(tk[i])) i++; if (i >= tk.size()) break; size_t s = i; while (i < tk.size() && !is_delim(tk[i])) i++;
+                if (i - s >= 3) P.terms->add_weighted(P.terms->key(sv(tk.data() + s, i - s)), d, fw_at(2 + (int)s)); }
             // prefix docsets (PositionalPrefixIndex over the index text)
             for (size_t i = 0; i < idx.size();) { while (i < idx.size() && is_delim(idx[i])) i++; if (i >= idx.size()) break; size_t s = i; while (i < idx.size() && !is_delim(idx[i])) i++;
                 size_t ml = std::min<size_t>(3, i - s); for (size_t l = 1; l <= ml; l++) P.prefix->add_doc(P.prefix->key(sv(idx.data() + s, l)), d); }
@@ -291,12 +336,16 @@ int ifx_builder_finish(ifx_builder* b, int threads) {
                     P.champs.push_back({ch, (uint16_t)((prec << 8) | base), d});
                 }
             }
-            // WordMatcher.Load / word-idf / metadata work on normalize(lower(IndexedText))
+            // WordMatcher.Load / word-idf / metadata work on normalize(lower(IndexedText)); with a map the metadata on its CanonicalizeText
+            // (VectorModel.cs:268-281), WordMatcher and word idf on the text as it is (SearchEngine.cs:143, VectorModel.cs:864-908)
             tmp = raw; lower_inplace(tmp); normalize_into(tmp, wm);
             int ntok = 0; bool first = true; seen_words.clear();
+            auto meta_word = [&](sv w) { ntok++; if (first) { P.ft.insert(P.ft.end(), w.begin(), w.end()); P.ft_len.push_back((uint32_t)w.size()); first = false; } };
+            if (syn) { canon_into(wm, meta, b->syn);
+                for (size_t i = 0; i < meta.size();) { while (i < meta.size() && is_delim(meta[i])) i++; if (i >= meta.size()) break; size_t s = i; while (i < meta.size() && !is_delim(meta[i])) i++; meta_word(sv(meta.data() + s, i - s)); } }
             for (size_t i = 0; i < wm.size();) { while (i < wm.size() && is_delim(wm[i])) i++; if (i >= wm.size()) break; size_t s = i; while (i < wm.size() && !is_delim(wm[i])) i++;
-                sv w(wm.data() + s, i - s); int len = (int)w.size(); ntok++;
-                if (first) { P.ft.insert(P.ft.end(), w.begin(), w.end()); P.ft_len.push_back((uint32_t)len); first = false; }
+                sv w(wm.data() + s, i - s); int len = (int)w.size();
+                if (!syn) meta_word(w);
                 if (len >= 2 && len <= 8) P.exact->add_doc(P.exact->key(w), d);
                 if (len >= 3 && len <= 8) for (int k = 0; k < len; k++) { tmp.assign(w); tmp.erase(k, 1); P.ld1->add_doc(P.ld1->key(tmp), d); }
                 if (len >= 3) { bool nw; int a = P.affix.intern(w, &nw); if (nw) P.affix_last.push_back(d); else P.affix_last[a] = d; }
@@ -397,6 +446,7 @@ int ifx_builder_finish(ifx_builder* b, int threads) {
     I.n_columns = (int)b->cols.size(); I.columns = b->cols.data();
     I.n_champ_chars = (int)b->champ_off.size() - 1; I.champ_chars = b->champ_chars.data(); I.champ_off = b->champ_off.data(); I.champ_doc = b->champ_doc.data(); I.champ_score = b->champ_score.data();
     I.n_raw = (int)b->raw_off.size() - 1; I.raw_doc = b->raw_doc.data(); I.raw_off = b->raw_off.data(); I.raw_chars = (const uint16_t*)b->raw_chars.data();
+    if (syn) { I.syn_keys = S(b->syn_key_chars, b->syn_key_off); I.syn_canon = S(b->syn_canon_chars, b->syn_canon_off); }
     // free the raw documents
     b->values.clear(); b->values.shrink_to_fit(); b->is_null.clear();
     b->finished = true; return IFX_OK;
@@ -527,6 +577,16 @@ extern "C" int ifx_host_prepare_query(const uint16_t* in, int n, uint16_t* out, 
     int b = 0, e = n; while (b < e && ws[in[b]]) b++; while (e > b && ws[in[e - 1]]) e--;
     str nrm; normalize_into(sv((const char16_t*)in + b, (size_t)(e - b)), nrm); lower_inplace(nrm);
     int m = (int)std::min<size_t>(nrm.size(), (size_t)cap); std::memcpy(out, nrm.data(), (size_t)m * 2);
+    return (int)nrm.size();
+}
+
+// SearchEngine.Search (SearchEngine.cs:264-288) up to the text SearchPipeline.Execute works on (its second Normalize, SearchPipeline.cs:68-71)
+extern "C" int ifx_builder_prepare_query(ifx_builder* b, const uint16_t* in, int n, uint16_t* out, int cap) {
+    if (!b || !b->has_syn()) return ifx_host_prepare_query(in, n, out, cap);
+    int b0 = 0, e = n; while (b0 < e && is_ws(in[b0])) b0++; while (e > b0 && is_ws(in[e - 1])) e--;
+    str nrm, cn; normalize_into(sv((const char16_t*)in + b0, (size_t)(e - b0)), nrm); lower_inplace(nrm);
+    canon_into(nrm, cn, b->syn); normalize_into(cn, nrm);
+    int m = (int)std::min<size_t>(nrm.size(), (size_t)std::max(cap, 0)); if (m) std::memcpy(out, nrm.data(), (size_t)m * 2);
     return (int)nrm.size();
 }
 

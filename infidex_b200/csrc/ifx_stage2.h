@@ -235,7 +235,7 @@ IFX_FN void cov_eval_entry(const DevIndex& ix, const QueryPlan& p, const Stage2B
     int lcs = 0;
     if (doc == B.di_doc[q * 2] || doc == B.di_doc[q * 2 + 1]) {
         int tol = cq.qlen >= 5 ? (int)((double)cq.qlen * 0.2) : 0;
-        int64_t t0 = ix.text_off[doc]; Str d{ix.text + t0, (int)(ix.text_off[doc + 1] - t0)};
+        int64_t t0 = ix.cov_text_off[doc]; Str d{ix.cov_text + t0, (int)(ix.cov_text_off[doc + 1] - t0)};
         lcs = lcs_metric(ix, Str{p.qtext, cq.qlen}, d, tol); if (lcs > 255) lcs = 255;
     }
     CovResult r = coverage_fusion(ix, cq, p.qtext, doc, lcs, B.ent_base[o]);

@@ -52,11 +52,11 @@ def shard_ranges(n_docs, world):
 class ShardedSearchEngine:
     """SearchEngine over one doc-id-range shard per rank. `device`: "cuda" (NCCL) or "cpu" (gloo + the kernel emulation, tests only)."""
 
-    def __init__(self, dist, device_index=0, _gpu_lib=None):
+    def __init__(self, dist, device_index=0, _gpu_lib=None, synonymMap=None):
         import torch
         self.dist, self.torch = dist, torch
         self.rank, self.world = dist.get_rank(), dist.get_world_size()
-        self.eng = E.SearchEngine(device=device_index, _gpu_lib=_gpu_lib)
+        self.eng = E.SearchEngine(device=device_index, _gpu_lib=_gpu_lib, synonymMap=synonymMap)      # every shard's builder gets the map's table
         self.dev = torch.device("cpu") if _gpu_lib else torch.device("cuda", device_index)
         self.exchange_ms = {"fuzzy_df": 0.0, "stage1": 0.0, "final": 0.0}
         self.host_ms = {}          # wall time of the phased C-ABI calls of this rank (kernels + their host side), download, merge pieces

@@ -19,6 +19,7 @@ import numpy as np
 
 from . import _build
 from .filter import Filter
+from .synonyms import SynonymMap
 
 PKG = os.path.dirname(os.path.abspath(__file__))
 
@@ -172,9 +173,14 @@ def _load_gpu(path=None):
 
 
 class SearchEngine:
-    """Drop-in for the reference's SearchEngine (config 400 = CreateDefault)."""
+    """Drop-in for the reference's SearchEngine (config 400 = CreateDefault), optionally with a SynonymMap (SearchEngine.cs:44-76).
 
-    def __init__(self, device=0, _gpu_lib=None):
+    With a map, documents and queries are canonicalised as the reference does. The index is built with the map's table as it is when
+    the documents are indexed; a Search after the map has changed raises (index again to use the new map)."""
+    _synonym_map = None
+    _syn_version = None         # SynonymMap._version the index was built with (None: no map, or no mappings)
+
+    def __init__(self, device=0, _gpu_lib=None, synonymMap=None):
         self._host = _load_host()
         self._gpu = _load_gpu(_gpu_lib)
         self._device = device
@@ -184,6 +190,11 @@ class SearchEngine:
         self._filters = {}
         self._columns = []      # (name, dict strings) of filter / facet columns, image order
         self._is_indexed = False
+        self._synonym_map = synonymMap
+
+    @property
+    def SynonymMap(self):
+        return self._synonym_map
 
     @staticmethod
     def CreateDefault(device=0, _gpu_lib=None):
@@ -233,8 +244,30 @@ class SearchEngine:
         w = np.array([f.Weight for f in schema], np.int32)
         fl = np.array([_field_flags(f) for f in schema], np.int32)
         self._builder = self._host.ifx_builder_create(len(schema), _p(nb), _p(no.astype(np.int32)), _p(w), _p(fl))
+        self._set_synonyms()
         self._add_columns(keys, columns)
         self._finish(schema, threads, upload)
+
+    def _set_synonyms(self):
+        """Hand the map's table (key, GetCanonical(key)) to the new builder and remember which state of the map it is."""
+        m = self._synonym_map
+        self._syn_version = None
+        if m is None or not m.HasCanonicalMappings:
+            return
+        table = m.canonical_table()
+        kb, ko = pack_strings([k for k, _ in table]); cb, co = pack_strings([c for _, c in table])
+        ko32, co32 = ko.astype(np.uint32), co.astype(np.uint32)
+        keys = _Strings(kb.ctypes.data, ko32.ctypes.data, len(table)); canon = _Strings(cb.ctypes.data, co32.ctypes.data, len(table))
+        rc = self._host.ifx_builder_set_synonyms(C.c_void_p(self._builder), C.byref(keys), C.byref(canon))
+        if rc:
+            raise NativeError("ifx_builder_set_synonyms failed (%d)" % rc)
+        self._syn_version = m._version
+
+    def _check_synonyms(self):
+        m = self._synonym_map
+        now = m._version if m is not None and m.HasCanonicalMappings else None
+        if now != self._syn_version:
+            raise RuntimeError("the SynonymMap changed after the documents were indexed: index them again to search with the new map")
 
     def _add_columns(self, keys, columns):
         n = len(keys)
@@ -273,6 +306,7 @@ class SearchEngine:
         w = np.array([f.Weight for f in schema], np.int32)
         fl = np.array([_field_flags(f) for f in schema], np.int32)
         self._builder = self._host.ifx_builder_create(len(schema), _p(nb), _p(no.astype(np.int32)), _p(w), _p(fl))
+        self._set_synonyms()
         for keys, columns in chunks:
             self._add_columns(np.ascontiguousarray(keys, np.int64), columns)
         self._finish(schema, threads)
@@ -292,8 +326,13 @@ class SearchEngine:
     # ---- searching --------------------------------------------------------------------------------------------------
     def _prep_text(self, text):
         a = np.frombuffer(text.encode("utf-16-le", "surrogatepass"), np.uint16) if text else np.zeros(0, np.uint16)
-        out = np.zeros(max(len(a), 1), np.uint16)
-        n = self._host.ifx_host_prepare_query(_p(np.ascontiguousarray(a)), len(a), _p(out), len(out))
+        a = np.ascontiguousarray(a); out = np.zeros(max(len(a), 1), np.uint16)
+        if self._syn_version is None:
+            n = self._host.ifx_host_prepare_query(_p(a), len(a), _p(out), len(out))
+            return out[:n]
+        n = self._host.ifx_builder_prepare_query(C.c_void_p(self._builder), _p(a), len(a), _p(out), len(out))
+        if n > len(out):            # a canonical form longer than its surface form
+            out = np.zeros(n, np.uint16); n = self._host.ifx_builder_prepare_query(C.c_void_p(self._builder), _p(a), len(a), _p(out), len(out))
         return out[:n]
 
     def _filter_id(self, flt):
@@ -346,6 +385,7 @@ class SearchEngine:
         return p
 
     def _pack_queries(self, queries):
+        self._check_synonyms()
         texts = [self._prep_text(q.Text) for q in queries]
         arr = (_Query * len(queries))()
         for i, q in enumerate(queries):

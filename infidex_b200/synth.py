@@ -150,3 +150,21 @@ def schema_and_columns(docs, multi_field):
               Field("rating", None, Weight.Med, indexable=False, filterable=True),
               Field("genre", None, Weight.Med, indexable=False, filterable=True, facetable=True)]
     return schema, [docs["title"], docs["description"], docs["year"], docs["rating"], genre]
+
+
+def make_synonym_pairs(vocab, n_groups=5000, seed=SEED, n_frequent=50):
+    """Seeded SynonymMap over the vocabulary: `n_groups` disjoint groups of 2-4 words of mixed lengths; the first groups take the
+    `n_frequent` most frequent words, the rest random ones. Returns the ordered AddSynonym(a, b) calls AddSynonymGroup(group) makes."""
+    rng = np.random.Generator(np.random.PCG64(seed ^ 0x5E5E))
+    words = vocab["words"]; V = len(words)
+    order = np.concatenate([np.arange(min(n_frequent, V)), rng.permutation(np.arange(min(n_frequent, V), V))])
+    pairs, k = [], 0
+    for g in range(n_groups):
+        size = int(rng.integers(2, 5))
+        grp = [words[int(i)] for i in order[k:k + size]]; k += size
+        if len(grp) < 2:
+            break
+        for i in range(len(grp)):
+            for j in range(i + 1, len(grp)):
+                pairs.append((grp[i], grp[j]))
+    return pairs
