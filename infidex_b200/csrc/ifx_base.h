@@ -43,6 +43,10 @@ constexpr int MAX_RAW_TOKENS = 128;  // VectorModel.cs:381 (ArrayPool rent of 12
 constexpr int MAX_TERMS = 128;
 constexpr int MAX_FUZZY = 16;        // unknown words (len >= 4) expanded per query
 #define IFX_QDBG 24                   // int64 slots of the per-query Stage-1 debug record (ifx_debug_stage1_queries)
+                                     // 0 candidates, 1 scored terms, 2 selection end (ns), 3 path, 4 select + lookup ns, 5 CTA, 6 lookup mode, 7 chunks,
+                                     // 8 largest chunk, 9 tf rows, 10 scorer ns, 11-15 lookup phase cycles and 20-23 selection cycles (-DIFX_S1_TIMERS),
+                                     // 18 AND tier 1: 0 not reached, 1 the id array saved by tier 0, recomputed because 2 a list is longer than the
+                                     // held-out one or 3 tier 0's last step ran on the bitset (not a timing)
 constexpr int LD1_CAP = 1024;        // VectorModel.cs:662 stackalloc int[1024]
 constexpr int CHUNK = 4096;          // Bm25Scorer.cs:209 blockSize
 constexpr int MAX_K = 1024;          // coverage depth supported by the on-chip heap

@@ -287,11 +287,18 @@ IFX_FN void warp_append(const Ctx& c, bool pred, int32_t value, int32_t* arr, in
 // unordered id array (ping-pong ws.buf_a / ws.buf_b) and as the membership bitset ws.bits2. Each further list either streams
 // past the bitset (coalesced, when it is not much longer than the running set) or is probed per surviving id (binary search).
 // Returns the size (-1: buffer overflow); `res` points at the surviving ids; ws.bits2 is left all-zero.
-IFX_FN int64_t intersect_terms(const Ctx& c, const DevIndex& ix, S1Workspace& ws, S1SelShared& sh, int cnt, const int32_t*& res) {
+// The AND of the first cnt - 1 terms (the next tier) comes for free when the held-out list sh.order[cnt - 1] sorts last by length (it
+// is at least as long as every other list: the insertion sort is stable and it is the last input), so the first cnt - 1 steps are
+// exactly those of a run with cnt - 1 (same seed, same order, same overflow rule), and that last step ran on the id array: the array
+// before it survives in the other ping-pong buffer. Then `res1` / `n1` hold that set; otherwise the caller recomputes it (n1 = -1: a
+// list is longer than the held-out one, -2: the last step ran on the bitset).
+IFX_FN int64_t intersect_terms(const Ctx& c, const DevIndex& ix, S1Workspace& ws, S1SelShared& sh, int cnt, const int32_t*& res, const int32_t*& res1, int64_t& n1) {
     const int NT = c.nthreads();
     int by_len[MAX_TERMS];
     for (int i = 0; i < cnt; i++) by_len[i] = sh.order[i];
     for (int i = 1; i < cnt; i++) { int x = by_len[i]; int j = i - 1; while (j >= 0 && sh.terms[by_len[j]].len > sh.terms[x].len) { by_len[j + 1] = by_len[j]; j--; } by_len[j + 1] = x; }
+    n1 = -1; res1 = nullptr;
+    const bool held_last = cnt >= 3 && by_len[cnt - 1] == sh.order[cnt - 1];
     const TermS& t0 = sh.terms[by_len[0]];
     int64_t n = t0.len; if (n > ws.buf_cap) return -1;
     int32_t* cur = ws.buf_a; int32_t* nxt = ws.buf_b;
@@ -335,13 +342,15 @@ IFX_FN int64_t intersect_terms(const Ctx& c, const DevIndex& ix, S1Workspace& ws
             const int64_t nbits = block_sum(c, mine, sh.scan);
             if (li + 1 < cnt && 16 * nbits < bw) { n = expand(false); li_start = li + 1; seeded = true; break; }      // bits2 keeps the membership: the invariant of the loop below
         }
-        if (!seeded) { const int64_t total = expand(true); res = cur; return total; }
+        if (!seeded) { const int64_t total = expand(true); res = cur; if (held_last) n1 = -2; return total; }      // the last step ran on the bitset: no next tier
     }
     if (!seeded) {
         for (int64_t i = c.tid(); i < n; i += NT) { int d = t0.docs[i]; cur[i] = d; if (cnt > 1) atomic_or(&ws.bits2[d >> 5], 1u << (d & 31)); }
         c.sync();
     }
+    if (held_last) { res1 = cur; n1 = 0; }      // stays empty unless the loop reaches the last list (a set that empties earlier is empty for the next tier too)
     for (int li = li_start; li < cnt && n > 0; li++) {
+        if (held_last && li == cnt - 1) { res1 = cur; n1 = n; }      // the last step writes `nxt` and only reads `cur`
         const TermS& t = sh.terms[by_len[li]];
         if (c.tid() == 0) sh.bcast[6] = 0;
         c.sync();
@@ -508,7 +517,7 @@ IFX_FN float bm25_scalar(float tf, float dl, float avgdl, float idf) {
     float core = (tf * (K1 + 1.f)) / denom; return idf * (core + Delta);
 }
 
-struct Stage1Out { int64_t* key; int32_t* doc; float* score; int32_t* n; long long* dbg; };   // dbg: [n_cand, n_terms, selection ns, path] or null   // row pointers for this query (cap = depth)
+struct Stage1Out { int64_t* key; int32_t* doc; float* score; int32_t* n; long long* dbg; };   // dbg: [n_cand, n_terms, selection ns, path, ...; 18: AND tier 1 route, see IFX_QDBG] or null   // row pointers for this query (cap = depth)
 
 // ---------------------------------------------------------------------------------------------------------------
 // LD1 expansion of one unknown word: first 1024 trie-order matches (Myers bit-vector, search variant), union of
@@ -651,7 +660,7 @@ IFX_FN int stage1_select(const Ctx& c, const DevIndex& ix, const QueryPlan& p, c
         for (int i = 0; i < n; i++) { const TermS& t = sh.terms[i]; if (t.term_id < 0 || t.idf <= 0.f) continue;      // (ids are unique within a query)
             unsigned h = qh_hash(t.term_id); while (sh.qh_key[h] >= 0) h = (h + 1) & (QH_SIZE - 1); sh.qh_key[h] = t.term_id; sh.qh_slot[h] = (uint8_t)i; }
         sh.n_terms = n; sh.streamed_mask[0] = sh.streamed_mask[1] = 0;
-        out.n[0] = 0;
+        out.n[0] = 0; if (out.dbg) out.dbg[18] = 0;
     }
     c.sync();
     const int T = sh.n_terms;
@@ -697,7 +706,7 @@ IFX_FN int stage1_select(const Ctx& c, const DevIndex& ix, const QueryPlan& p, c
             }
         } else {
             if (c.tid() == 0) for (int i = 0; i < T; i++) sh.streamed_mask[i >> 6] |= 1ULL << (i & 63);   // every list of the AND tier
-            const int32_t* r0 = nullptr; int64_t n0 = intersect_terms(c, ix, ws, sh, T, r0);
+            const int32_t* r0 = nullptr; const int32_t* r1 = nullptr; int64_t n1 = -1; int64_t n0 = intersect_terms(c, ix, ws, sh, T, r0, r1, n1);
             if (n0 < 0) { if (c.tid() == 0) out.n[0] = -1; return -1; }
             g += or_list_into_bits(c, r0, n0, ws, sh);
             IFX_STICK(1);   // AND tier 0
@@ -705,7 +714,10 @@ IFX_FN int stage1_select(const Ctx& c, const DevIndex& ix, const QueryPlan& p, c
             int64_t G = smode == 2 ? (int64_t)cnt[0] : g; if (smode == 1 && c.tid() == 0) { cnt[0] = (int32_t)g; cnt[1] = cnt[2] = cnt[3] = (int32_t)g; }
             if (smode == 1 && g >= (int64_t)K * 2) certain = true;          // tier 0 alone is enough on this shard, hence in the corpus
             if (G < (int64_t)K * 2) {
-                if (T >= 3 && G < (int64_t)K * 3) { const int32_t* r1 = nullptr; int64_t n1 = intersect_terms(c, ix, ws, sh, T - 1, r1); if (n1 > 0) g += or_list_into_bits(c, r1, n1, ws, sh); }
+                if (T >= 3 && G < (int64_t)K * 3) {      // tier 1: every list but the lowest-idf one -- saved by tier 0's intersection when it could be
+                    if (c.tid() == 0 && out.dbg) out.dbg[18] = n1 >= 0 ? 1 : (n1 == -1 ? 2 : 3);
+                    if (n1 < 0) { const int32_t* u = nullptr; int64_t nu = -1; n1 = intersect_terms(c, ix, ws, sh, T - 1, r1, u, nu); }
+                    if (n1 > 0) g += or_list_into_bits(c, r1, n1, ws, sh); }
                 IFX_STICK(2);   // AND tier 1
                 G = smode == 2 ? (int64_t)cnt[1] : g; if (smode == 1 && c.tid() == 0) { cnt[1] = (int32_t)g; cnt[2] = cnt[3] = (int32_t)g; }
                 if (G < (int64_t)K * 5) {

@@ -19,6 +19,7 @@ for i in order[:12]:
     print("%-40s cand=%8d T=%3d path=%d sel=%.2fms total=%.2fms cta=%d" % (qs[i][:40], dbg[i, 0], dbg[i, 1], dbg[i, 3], dbg[i, 2] / 1e6, dbg[i, 4] / 1e6, dbg[i, 5]))
 ph = dbg[:, 6:11].sum(0); print("scoring cycles share (thread 0 = heap warp): wait-for-workers %.1f%% eligibility+compaction %.1f%% phaseA(later tiles) %.1f%% phaseB %.1f%% heap drain %.1f%%" % tuple(100 * ph / ph.sum()), "| scoring cycles total %.0f M" % (ph.sum() / 1e6))
 for i in order[:8]: print("   ", qs[i][:30], (dbg[i, 6:11] / 1e3).astype(int), "kcycles", "eligible", dbg[i, 11] & 0xFFFFF, "heap updates", dbg[i, 11] >> 20)
+dbg[:, 18] = 0      # slot 18 is the AND tier-1 route code (ifx_base.h IFX_QDBG), not a timing
 wp = dbg[:, 12:20].sum(0); print("worker-view cycles share: ids+norms %.1f%% bounds %.1f%% bitmap %.1f%% phaseA0 %.1f%% join-wait %.1f%% phaseA-later %.1f%% its-barrier %.1f%% post-join(B+elig) %.1f%%" % tuple(100 * wp / wp.sum()))
 for i in order[:8]: print("   W", qs[i][:30], (dbg[i, 12:20] / 1e3).astype(int), "kcycles")
 for i in order[:8]: print("   S", qs[i][:30], (dbg[i, 20:24] / 1e3).astype(int), "kcycles [prefix+sort, tier0/unions, tier1, compact]")
