@@ -89,7 +89,6 @@ struct DevIndex {
     int32_t n_cont;                  // 65536-doc containers in this shard
     const int32_t* bm_id;            // per term: row of the dense-term bitmap table, or -1
     const unsigned* bm_bits;         // [n_bm][bm_words] membership bitmap of the posting list (dense terms: df >= n_docs / 32)
-    const int32_t* bm_rank;          // [n_bm][bm_words] postings before doc (w << 5): posting index = rank[w] + popc(bits[w] & (bit - 1))
     int32_t bm_words;
     StrDict words; const float* word_idf;
     DocsetDict prefix, wm_exact, wm_ld1;
@@ -248,7 +247,7 @@ struct QueryPlan {
     FuzzyReq fuzzy[MAX_FUZZY];
 };
 
-struct BatchCounters { int32_t n_fuzzy_items; int32_t overflow; unsigned long long fuzzy_pool_used; unsigned long long algo_bytes; unsigned long long s1_ns_sum; unsigned long long s1_ns_max; unsigned long long s1_cand_sum;
+struct BatchCounters { int32_t n_fuzzy_items; int32_t overflow; unsigned long long fuzzy_pool_used; unsigned long long algo_bytes; unsigned long long s1_ns_sum; unsigned long long s1_ns_max;
                        unsigned long long s1_pool_used; int32_t s1_deferred, s1_n_light, s1_n_heavy, s1_wave, s1_n_mid, n_short;
                        int32_t n_tf_pairs, n_tf_groups; };     // the wave's term-major tf lookups: TfPairs appended by stage1_lookup, distinct terms among them
 

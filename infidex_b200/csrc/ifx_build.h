@@ -75,22 +75,11 @@ IFX_GLOBAL void IFX_BOUNDS(256) k_skip_table(const int64_t* row_ptr, const int32
     skip_ptr[idx] = (int32_t)(lower_bound_i32(post_doc, row_ptr[t], row_ptr[t + 1], cb << 16) - row_ptr[t]);
 }
 
-// ---- dense-term bitmaps + rank directories: one block per dense row ---------------------------------------------------------
+// ---- dense-term bitmaps: one block per dense row ---------------------------------------------------------
 IFX_GLOBAL void IFX_BOUNDS(512) k_bitmap_fill(const int64_t* row_ptr, const int32_t* bm_terms, int bm_words, const int32_t* post_doc, unsigned* bm_bits) {
     Ctx c; const int t = bm_terms[c.block()]; unsigned* b = bm_bits + (size_t)c.block() * bm_words;
     const int64_t r0 = row_ptr[t], r1 = row_ptr[t + 1];
     for (int64_t i = r0 + c.tid(); i < r1; i += (unsigned)c.nthreads()) { int d = post_doc[i]; atomic_or(&b[d >> 5], 1u << (d & 31)); }
-}
-IFX_GLOBAL void IFX_BOUNDS(512) k_bitmap_rank(int bm_words, const unsigned* bm_bits, int32_t* bm_rank) {
-    IFX_SHARED ScanTmpT<unsigned long long> wt; Ctx c;
-    const unsigned* b = bm_bits + (size_t)c.block() * bm_words; int32_t* r = bm_rank + (size_t)c.block() * bm_words; unsigned long long run = 0;
-    for (int w0 = 0; w0 < bm_words; w0 += 4 * c.nthreads()) {
-        const int wb = w0 + c.tid() * 4; unsigned v[4]; unsigned long long s = 0;
-        for (int u = 0; u < 4; u++) { v[u] = wb + u < bm_words ? b[wb + u] : 0u; s += popc(v[u]); }
-        unsigned long long tot; unsigned long long ex = run + block_excl_scan(c, s, wt, tot);
-        for (int u = 0; u < 4; u++) { if (wb + u < bm_words) r[wb + u] = (int32_t)ex; ex += popc(v[u]); }
-        run += tot;
-    }
 }
 
 // ---- coverage text of an index with a SynonymMap: SynonymMap.CanonicalizeText(Normalize(IndexedText)) per document, one thread each --

@@ -178,20 +178,20 @@ IFX_FN int64_t warp_lower_bound(const Ctx& c, const int32_t* a, int64_t lo, int6
 
 // per-CTA global workspace
 struct S1Workspace {
-    unsigned* bits;        // candidate bitset over the shard's docs (all zero between uses)
+    unsigned* bits;        // candidate bitset over the shard's docs (the candidate-set section below)
     unsigned* bits2;       // membership bitset of the running AND-tier intersection (all zero between uses)
-    int32_t* cand;         // sorted candidate ids
+    unsigned* wm_sum;      // wm_query's summary of `bits`: one bit per word its union touched (all zero between uses)
     int32_t* buf_a; int32_t* buf_b;   // AND-tier ping-pong arrays
     unsigned long long* surv_g;       // [CHUNK] flush survivors of one chunk when they exceed the shared staging buffer
     int32_t* loff;         // [n_cont + 1][streamed lists] offset of the first posting of each streamed list in container c (scratch of the tf lookups)
     int32_t* cstart;       // [n_cont + 1] candidates before container c
     int32_t* cfirst;       // [n_cont + 1] chunks before container c
     int32_t* cpad;         // [n_cont + 1] padded tf slots before container c
-    int64_t cand_cap, buf_cap;
+    int64_t buf_cap;
 };
 
 struct TermS {             // term as seen by the scorer
-    const int32_t* docs; const uint8_t* tf; const int32_t* skip; const unsigned* bm; const int32_t* bmr; int32_t len; int32_t df; float idf, max_score, suffix_after; int32_t term_id; int64_t cursor, s0, s1;
+    const int32_t* docs; const uint8_t* tf; const int32_t* skip; const unsigned* bm; int32_t len; int32_t df; float idf, max_score, suffix_after; int32_t term_id;
 };
 
 constexpr int S1_TILE = 6;
@@ -207,7 +207,7 @@ struct S1SelShared {
     int order[MAX_TERMS];
     int n_terms;
     int32_t qh_key[QH_SIZE]; uint8_t qh_slot[QH_SIZE];   // term id -> slot in `terms` (open addressing; terms with idf > 0 only), for the forward-index lookups
-    uint8_t dirty[MAX_CONTAINERS];          // containers of the global bitset touched by the current set operation (all zero between uses)
+    uint8_t dirty[MAX_CONTAINERS];          // the candidate set's container flags (the candidate-set section below)
     ScanTmp scan; ScanTmp scan2[2];
     int bcast[8]; long long bcast64[4];
     unsigned long long streamed_mask[2];   // terms whose list the selector streamed in full (roofline accounting)
@@ -266,12 +266,82 @@ IFX_FN void stream_list_words(const Ctx& c, const int32_t* list, int64_t n, Put 
     }
 }
 
-// OR a sorted id list into the CTA's bitset; returns the number of newly set docs (block-wide).
-IFX_FN int or_list_into_bits(const Ctx& c, const int32_t* list, int64_t n, S1Workspace& ws, S1SelShared& sh) {
+// ---------------------------------------------------------------------------------------------------------------
+// The CTA's candidate set: ws.bits, one bit per document of the shard (allocated and zero up to whole containers), plus `dirty` in
+// shared memory, one flag per 65 536-doc container (2048 words) that may hold set bits. Both are all-zero whenever the CTA is between
+// two uses: a kernel zeroes the flags at entry (cand_init), and every use ends with cand_clear. Two readers zero the words as they
+// read them (the tf lookups' container window, wm_query's ordered walk) and then reset only the flags (cand_clear, words_zeroed).
+
+IFX_FN void cand_init(const Ctx& c, uint8_t* dirty) {      // kernel entry: shared memory starts undefined
+    for (int i = c.tid(); i < MAX_CONTAINERS; i += (unsigned)c.nthreads()) dirty[i] = 0;
+    c.sync();
+}
+
+// OR a sorted id list into the set; returns the number of newly set docs (block-wide).
+IFX_FN int cand_or_list(const Ctx& c, const int32_t* list, int64_t n, S1Workspace& ws, S1SelShared& sh) {
     int fresh = 0;
     stream_list_words(c, list, n, [&](int word, unsigned mask) { unsigned old = atomic_or(&ws.bits[word], mask); fresh += popc(mask & ~old); sh.dirty[word >> 11] = 1; });
     c.sync();
     return block_sum(c, fresh, sh.scan);
+}
+
+// Add one document (any thread); true when it was not in the set yet.
+IFX_FN bool cand_add(S1Workspace& ws, uint8_t* dirty, int d) {
+    const unsigned bit = 1u << (d & 31); const unsigned old = atomic_or(&ws.bits[d >> 5], bit);
+    dirty[d >> 16] = 1;
+    return !(old & bit);
+}
+
+// Each warp owns a contiguous span [w0, w1) of the bitset's words (whole 32-word groups), so the expansion comes out ascending;
+// `base`: the documents before the span. cand_count fills it for cand_expand.
+struct CandSpan { int64_t w0, w1; int base; };
+
+// Size of the set (block-wide; non-dirty containers are skipped).
+IFX_FN int cand_count(const Ctx& c, const DevIndex& ix, const S1Workspace& ws, S1SelShared& sh, CandSpan& sp) {
+    constexpr int WS = Ctx::WS; const int NW = c.nwarps(); const int64_t nwords = ((int64_t)ix.n_docs + 31) >> 5;
+    const int64_t span = (((nwords + NW - 1) / NW) + 31) / 32 * 32; const int64_t w0 = (int64_t)c.warp() * span, w1 = w0 + span < nwords ? w0 + span : nwords;
+    int mycnt = 0;
+    for (int64_t g0 = w0; g0 < w1; g0 += 4 * WS) {      // four groups (independent loads) per trip
+        unsigned v[4];
+        for (int u = 0; u < 4; u++) { const int64_t g = g0 + u * WS, w = g + c.lane(); v[u] = (g < w1 && sh.dirty[g >> 11] && w < w1) ? ws.bits[w] : 0u; }
+        for (int u = 0; u < 4; u++) mycnt += popc(v[u]);
+    }
+    int n; const int ex0 = block_excl_scan(c, mycnt, sh.scan, n);
+    sp.w0 = w0; sp.w1 = w1; sp.base = c.shfl(ex0, 0);
+    return n;
+}
+
+// The set's `n` documents (cand_count) in ascending order into out[0, n), and ws.cstart[k] = documents before container k (k <= n_cont).
+// The set is left as it is.
+IFX_FN void cand_expand(const Ctx& c, const DevIndex& ix, S1Workspace& ws, const S1SelShared& sh, const CandSpan& sp, int n, int32_t* out) {
+    constexpr int WS = Ctx::WS; const int64_t w0 = sp.w0, w1 = sp.w1;
+    int run = sp.base;
+    for (int64_t gb = w0; gb < w1; gb += 4 * WS) {          // four groups per trip: their words are loaded together, then scanned one after the other
+        unsigned vv[4];
+        for (int u = 0; u < 4; u++) { const int64_t g = gb + u * WS, w = g + c.lane(); vv[u] = (g < w1 && sh.dirty[g >> 11] && w < w1) ? ws.bits[w] : 0u; }
+        for (int u = 0; u < 4; u++) {
+            const int64_t g0 = gb + u * WS; if (g0 >= w1) break;
+            if (!sh.dirty[g0 >> 11]) { if ((g0 & 2047) == 0 && c.lane() == 0) ws.cstart[g0 >> 11] = run; continue; }
+            const int64_t w = g0 + c.lane(); unsigned v = vv[u]; const int pc = popc(v); int incl = pc;
+            for (int d = 1; d < WS; d <<= 1) { int o = c.shfl(incl, c.lane() >= d ? c.lane() - d : 0); if (c.lane() >= d) incl += o; }
+            int o = run + incl - pc;
+            if (w < w1 && (w & 2047) == 0) ws.cstart[w >> 11] = o;
+            while (v) { int b = ffs32(v) - 1; v &= v - 1; out[o++] = (int32_t)((w << 5) | b); }
+            run += c.shfl(incl, WS - 1);
+        }
+    }
+    if (c.tid() == 0) ws.cstart[(ix.n_docs + 65535) >> 16] = n;
+    c.sync();
+}
+
+// The set back to all-zero: the words of the dirty containers (unless a reader has zeroed them already), then the flags.
+IFX_FN void cand_clear(const Ctx& c, const DevIndex& ix, S1Workspace& ws, uint8_t* dirty, bool words_zeroed = false) {
+    const int NT = c.nthreads(); const int64_t nwords = ((int64_t)ix.n_docs + 31) >> 5; const int ncont = (ix.n_docs + 65535) >> 16;
+    c.sync();
+    if (!words_zeroed) for (int64_t w = c.tid(); w < nwords; w += NT) if (dirty[w >> 11]) ws.bits[w] = 0u;
+    c.sync();
+    for (int k = c.tid(); k < ncont; k += NT) dirty[k] = 0;
+    c.sync();
 }
 
 // Warp-aggregated unordered append (all lanes of the warp must call it together).
@@ -388,29 +458,6 @@ IFX_FN int64_t intersect_terms(const Ctx& c, const DevIndex& ix, S1Workspace& ws
     res = cur;
     c.sync();
     return n;
-}
-
-// Expand the dirty containers of the bitset into ws.cand (ascending) and clear them. Returns the count.
-IFX_FN int64_t compact_bits(const Ctx& c, const DevIndex& ix, S1Workspace& ws, S1SelShared& sh, int32_t* out, int64_t out_cap, bool& overflow) {
-    int ncont = (ix.n_docs + 65535) >> 16; int64_t total = 0; int64_t nwords = ((int64_t)ix.n_docs + 31) >> 5;
-    overflow = false;
-    for (int k = 0; k < ncont; k++) {
-        if (!sh.dirty[k]) continue;                    // uniform across the CTA (shared flag, synced by callers)
-        int64_t w0 = (int64_t)k * 2048, w1 = w0 + 2048; if (w1 > nwords) w1 = nwords;
-        int per = (int)((w1 - w0 + c.nthreads() - 1) / c.nthreads());
-        int64_t my0 = w0 + (int64_t)c.tid() * per, my1 = my0 + per; if (my1 > w1) my1 = w1;
-        int cnt = 0; for (int64_t w = my0; w < my1; w++) cnt += popc(ws.bits[w]);
-        int tot; int off = block_excl_scan(c, cnt, sh.scan, tot);
-        if (total + tot > out_cap) { overflow = true; }
-        else { int64_t o = total + off;
-            for (int64_t w = my0; w < my1; w++) { unsigned v = ws.bits[w]; while (v) { int b = ffs32(v) - 1; out[o++] = (int32_t)((w << 5) | b); v &= v - 1; } } }
-        for (int64_t w = my0; w < my1; w++) ws.bits[w] = 0;
-        total += tot;
-        c.sync();
-        if (c.tid() == 0) sh.dirty[k] = 0;
-    }
-    c.sync();
-    return total;
 }
 
 // .NET ArraySortHelper<T>.IntrospectiveSort(keys, Comparison<T>) over element indices -- unstable, reproduced exactly because the tie
@@ -592,27 +639,24 @@ IFX_FN void expand_fuzzy(const Ctx& c, const DevIndex& ix, QueryPlan& p, int fsl
         int ord = matches[k]; if (ix.df[ord] <= 0) continue;
         int64_t r0 = ix.row_ptr[ord], r1 = ix.row_ptr[ord + 1];
         if (r1 - r0 >= BIG) { int slot = BIGQ; if (c.lane() == 0) slot = atomic_add(&sh.bcast[5], 1); slot = c.shfl(slot, 0); if (slot < BIGQ) { if (c.lane() == 0) sh.bprefix[slot] = ord; continue; } }
-        for (int64_t i = r0 + c.lane(); i < r1; i += Ctx::WS) {
-            int d = ix.post_doc[i]; unsigned bit = 1u << (d & 31);
-            unsigned old = atomic_or(&ws.bits[d >> 5], bit);
-            if (!(old & bit)) fresh++;
-            sh.dirty[d >> 16] = 1;
-        }
+        for (int64_t i = r0 + c.lane(); i < r1; i += Ctx::WS) if (cand_add(ws, sh.dirty, ix.post_doc[i])) fresh++;
     }
     c.sync();
     int df = block_sum(c, fresh, sh.scan);
     const int nbig = sh.bcast[5] < BIGQ ? sh.bcast[5] : BIGQ;
-    for (int k = 0; k < nbig; k++) { int ord = sh.bprefix[k]; int64_t r0 = ix.row_ptr[ord], r1 = ix.row_ptr[ord + 1]; df += or_list_into_bits(c, ix.post_doc + r0, r1 - r0, ws, sh); }
+    for (int k = 0; k < nbig; k++) { int ord = sh.bprefix[k]; int64_t r0 = ix.row_ptr[ord], r1 = ix.row_ptr[ord + 1]; df += cand_or_list(c, ix.post_doc + r0, r1 - r0, ws, sh); }
     c.sync();
     QTerm& t = p.terms[fr.term_slot];
     if (df == 0) { if (c.tid() == 0) { t.df = 0; t.list_len = 0; } c.sync(); return; }
     if (c.tid() == 0) { unsigned long long b = atomic_add64(&bc->fuzzy_pool_used, (unsigned long long)df); sh.bcast64[0] = (long long)b; }
     c.sync();
-    unsigned long long b = (unsigned long long)sh.bcast64[0]; bool ovf = false;
-    int64_t cap = b + (unsigned long long)df <= pool_cap ? df : 0;
-    int64_t n = compact_bits(c, ix, ws, sh, pool + b, cap, ovf);
+    const unsigned long long b = (unsigned long long)sh.bcast64[0];
+    CandSpan sp; const int n = cand_count(c, ix, ws, sh, sp);
+    const bool fits = n == df && b + (unsigned long long)df <= pool_cap;      // the union fits the pool (and its size agrees with the fresh bits)
+    if (fits) cand_expand(c, ix, ws, sh, sp, n, pool + b);
+    cand_clear(c, ix, ws, sh.dirty);
     if (c.tid() == 0) {
-        if (ovf || n != df) { p.status |= 4; atomic_add(&bc->overflow, 1); t.df = 0; t.list_len = 0; }
+        if (!fits) { p.status |= 4; atomic_add(&bc->overflow, 1); t.df = 0; t.list_len = 0; }
         else { float avgdl = ix.avgdl > 0.f ? ix.avgdl : 1.f; t.df = df; t.list_len = df; t.list_off = (int64_t)b; t.idf = compute_idf(ix, df); t.max_score = max_term_score(t.idf, avgdl); }
     }
     c.sync();
@@ -649,10 +693,10 @@ IFX_FN int stage1_select(const Ctx& c, const DevIndex& ix, const QueryPlan& p, c
         for (int i = 0; i < p.n_terms; i++) {
             const QTerm& q = p.terms[i];
             if (q.df <= 0 || q.df > ix.stop_term_limit) continue;      // VectorModel.cs:521
-            TermS& t = sh.terms[n]; t.len = q.list_len; t.df = q.df; t.idf = q.idf; t.max_score = q.max_score; t.cursor = 0; t.term_id = q.term_id;
+            TermS& t = sh.terms[n]; t.len = q.list_len; t.df = q.df; t.idf = q.idf; t.max_score = q.max_score; t.term_id = q.term_id;
             if (q.term_id >= 0) { t.docs = ix.post_doc + q.list_off; t.tf = ix.post_tf + q.list_off; int sk = ix.skip_id[q.term_id]; t.skip = sk >= 0 ? ix.skip_ptr + (size_t)sk * (ix.n_cont + 1) : nullptr;
-                int bi = ix.bm_id[q.term_id]; t.bm = bi >= 0 ? ix.bm_bits + (size_t)bi * ix.bm_words : nullptr; t.bmr = bi >= 0 ? ix.bm_rank + (size_t)bi * ix.bm_words : nullptr; }
-            else { t.docs = pool + q.list_off; t.tf = nullptr; t.skip = nullptr; t.bm = nullptr; t.bmr = nullptr; }
+                int bi = ix.bm_id[q.term_id]; t.bm = bi >= 0 ? ix.bm_bits + (size_t)bi * ix.bm_words : nullptr; }
+            else { t.docs = pool + q.list_off; t.tf = nullptr; t.skip = nullptr; t.bm = nullptr; }
             n++;
         }
         float suf = 0.f; for (int i = n - 1; i >= 0; i--) { sh.terms[i].suffix_after = suf; suf = suf + sh.terms[i].max_score; }   // ComputeSuffixSums
@@ -676,7 +720,7 @@ IFX_FN int stage1_select(const Ctx& c, const DevIndex& ix, const QueryPlan& p, c
     int path = 0; bool certain = false;
     if (c.tid() == 0) { sh.bcast64[0] = -1; sh.bcast64[1] = 0; int64_t r0, pop; if (prefix_shortcut(ix, p, K, r0, pop)) { sh.bcast64[0] = r0; sh.bcast64[1] = pop; } }
     c.sync();
-    if (sh.bcast64[0] >= 0) { path = 1; certain = true; or_list_into_bits(c, ix.prefix.doc_id + sh.bcast64[0], sh.bcast64[1], ws, sh); }      // (the prefix rules read replicated corpus-level cardinalities)
+    if (sh.bcast64[0] >= 0) { path = 1; certain = true; cand_or_list(c, ix.prefix.doc_id + sh.bcast64[0], sh.bcast64[1], ws, sh); }      // (the prefix rules read replicated corpus-level cardinalities)
     else {
         if (c.tid() == 0) {
             bool typo = false; float max_idf = 0.f;
@@ -694,7 +738,7 @@ IFX_FN int stage1_select(const Ctx& c, const DevIndex& ix, const QueryPlan& p, c
                 const TermS& t = sh.terms[sh.order[oi]];
                 bool lowq = t.idf < (max_idf * 0.2f);
                 if (T > 1 && lowq && selective) continue;
-                g += or_list_into_bits(c, t.docs, t.len, ws, sh);
+                g += cand_or_list(c, t.docs, t.len, ws, sh);
                 if (c.tid() == 0) sh.streamed_mask[sh.order[oi] >> 6] |= 1ULL << (sh.order[oi] & 63);
                 int64_t gg = g;                                                   // the union's size over the whole corpus decides
                 if (smode == 1 && li < 32) { if (c.tid() == 0) cnt[8 + li] = (int32_t)g; if (t.df > df_max) df_max = t.df; gg = df_max;      // count pass: go on until the union certainly holds 100 K documents (it contains its largest list)
@@ -708,7 +752,7 @@ IFX_FN int stage1_select(const Ctx& c, const DevIndex& ix, const QueryPlan& p, c
             if (c.tid() == 0) for (int i = 0; i < T; i++) sh.streamed_mask[i >> 6] |= 1ULL << (i & 63);   // every list of the AND tier
             const int32_t* r0 = nullptr; const int32_t* r1 = nullptr; int64_t n1 = -1; int64_t n0 = intersect_terms(c, ix, ws, sh, T, r0, r1, n1);
             if (n0 < 0) { if (c.tid() == 0) out.n[0] = -1; return -1; }
-            g += or_list_into_bits(c, r0, n0, ws, sh);
+            g += cand_or_list(c, r0, n0, ws, sh);
             IFX_STICK(1);   // AND tier 0
             // count pass: a shard that alone reaches a limit knows the corpus does; below it every later stage is counted (some shard may need it)
             int64_t G = smode == 2 ? (int64_t)cnt[0] : g; if (smode == 1 && c.tid() == 0) { cnt[0] = (int32_t)g; cnt[1] = cnt[2] = cnt[3] = (int32_t)g; }
@@ -717,13 +761,13 @@ IFX_FN int stage1_select(const Ctx& c, const DevIndex& ix, const QueryPlan& p, c
                 if (T >= 3 && G < (int64_t)K * 3) {      // tier 1: every list but the lowest-idf one -- saved by tier 0's intersection when it could be
                     if (c.tid() == 0 && out.dbg) out.dbg[18] = n1 >= 0 ? 1 : (n1 == -1 ? 2 : 3);
                     if (n1 < 0) { const int32_t* u = nullptr; int64_t nu = -1; n1 = intersect_terms(c, ix, ws, sh, T - 1, r1, u, nu); }
-                    if (n1 > 0) g += or_list_into_bits(c, r1, n1, ws, sh); }
+                    if (n1 > 0) g += cand_or_list(c, r1, n1, ws, sh); }
                 IFX_STICK(2);   // AND tier 1
                 G = smode == 2 ? (int64_t)cnt[1] : g; if (smode == 1 && c.tid() == 0) { cnt[1] = (int32_t)g; cnt[2] = cnt[3] = (int32_t)g; }
                 if (G < (int64_t)K * 5) {
                     int sel[2]; int ns = 0; float cutoff = max_idf * 0.3f; int capn = T < 2 ? T : 2;
                     for (int oi = 0; oi < T && ns < capn; oi++) { const TermS& t = sh.terms[sh.order[oi]]; if (t.idf <= 0.f) continue; if (t.idf < cutoff) continue; sel[ns++] = sh.order[oi]; }
-                    for (int si = 0; si < ns; si++) { const TermS& t = sh.terms[sel[si]]; g += or_list_into_bits(c, t.docs, t.len, ws, sh);
+                    for (int si = 0; si < ns; si++) { const TermS& t = sh.terms[sel[si]]; g += cand_or_list(c, t.docs, t.len, ws, sh);
                         G = smode == 2 ? (int64_t)cnt[2 + si] : g; if (smode == 1 && c.tid() == 0) { cnt[2 + si] = (int32_t)g; if (si == 0) cnt[3] = (int32_t)g; }
                         if (G >= (int64_t)K * 10) break; }
                 }
@@ -739,16 +783,6 @@ IFX_FN int stage1_select(const Ctx& c, const DevIndex& ix, const QueryPlan& p, c
 #endif
     }
     return path;
-}
-
-// Candidate bitset back to all-zero (dirty containers only).
-IFX_FN void stage1_clear_bits(const Ctx& c, const DevIndex& ix, S1Workspace& ws, S1SelShared& sh) {
-    const int NT = c.nthreads(); const int64_t nwords = ((int64_t)ix.n_docs + 31) >> 5; const int ncont = (ix.n_docs + 65535) >> 16;
-    c.sync();
-    for (int64_t w = c.tid(); w < nwords; w += NT) if (sh.dirty[w >> 11]) ws.bits[w] = 0u;
-    c.sync();
-    for (int k = c.tid(); k < ncont; k += NT) sh.dirty[k] = 0;
-    c.sync();
 }
 
 }  // namespace ifx

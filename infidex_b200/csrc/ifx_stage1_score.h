@@ -54,53 +54,23 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
 #define IFX_LTICK(k) do { } while (0)
 #endif
     if (path <= 0) { if (c.tid() == 0) { rec.state = path < 0 ? -1 : 0; rec.n_cand = 0; rec.K = p.depth; rec.path = path; } c.sync(); return; }
-    const int T = sh.n_terms; const int64_t nwords = ((int64_t)ix.n_docs + 31) >> 5; const int ncont = (ix.n_docs + 65535) >> 16;
-    // ---- 1a. count (each warp owns a contiguous span of bitset words; non-dirty containers are skipped)
-    const int64_t span = (((nwords + NW - 1) / NW) + 31) / 32 * 32; const int64_t w0 = (int64_t)c.warp() * span, w1 = w0 + span < nwords ? w0 + span : nwords;
-    int mycnt = 0;
-    for (int64_t g0 = w0; g0 < w1; g0 += 4 * WS) {      // four groups (independent loads) per trip
-        unsigned v[4];
-        for (int u = 0; u < 4; u++) { const int64_t g = g0 + u * WS, w = g + c.lane(); v[u] = (g < w1 && sh.dirty[g >> 11] && w < w1) ? ws.bits[w] : 0u; }
-        for (int u = 0; u < 4; u++) mycnt += popc(v[u]);
-    }
-    int n_cand; int ex0 = block_excl_scan(c, mycnt, sh.scan, n_cand); const int wbase = c.shfl(ex0, 0);
-    auto clear_bits = [&](bool words) {      // words == false: the container walk of the tf lookups has zeroed them already
-        if (words) for (int64_t w = c.tid(); w < nwords; w += NT) if (sh.dirty[w >> 11]) ws.bits[w] = 0u;
-        c.sync();
-        for (int k = c.tid(); k < ncont; k += NT) sh.dirty[k] = 0;
-        c.sync();
-    };
-    if (n_cand == 0) { clear_bits(true); if (c.tid() == 0) { rec.state = 0; rec.n_cand = 0; rec.K = p.depth; rec.path = path; if (out.dbg) out.dbg[0] = 0; } c.sync(); return; }
+    const int T = sh.n_terms; const int ncont = (ix.n_docs + 65535) >> 16;
+    // ---- 1a. count
+    CandSpan sp; const int n_cand = cand_count(c, ix, ws, sh, sp);
+    if (n_cand == 0) { cand_clear(c, ix, ws, sh.dirty); if (c.tid() == 0) { rec.state = 0; rec.n_cand = 0; rec.K = p.depth; rec.path = path; if (out.dbg) out.dbg[0] = 0; } c.sync(); return; }
     auto pool_alloc = [&](unsigned long long bytes) -> long long {      // block-uniform result; -1: does not fit now, -2: can never fit
         if (c.tid() == 0) { long long r; bytes = (bytes + 255ULL) & ~255ULL;
             if (bytes > spool_cap) r = -2; else { unsigned long long at = atomic_add64(&bc->s1_pool_used, bytes); r = at + bytes <= spool_cap ? (long long)at : -1; }
             sh.bcast64[2] = r; }
         c.sync(); long long r = sh.bcast64[2]; c.sync(); return r;
     };
-    auto give_up = [&](long long why) { clear_bits(true); if (c.tid() == 0) { rec.state = why == -2 ? -1 : 2; rec.n_cand = n_cand; rec.K = p.depth; rec.path = path; if (why != -2) atomic_add(&bc->s1_deferred, 1); else out.n[0] = -1; } c.sync(); };      // a query larger than the whole pool is an overflow, like every other fixed buffer
+    auto give_up = [&](long long why) { cand_clear(c, ix, ws, sh.dirty); if (c.tid() == 0) { rec.state = why == -2 ? -1 : 2; rec.n_cand = n_cand; rec.K = p.depth; rec.path = path; if (why != -2) atomic_add(&bc->s1_deferred, 1); else out.n[0] = -1; } c.sync(); };      // a query larger than the whole pool is an overflow, like every other fixed buffer
     const unsigned long long a1_bytes = 8ULL * (unsigned long long)n_cand + 64;
     const long long a1 = pool_alloc(a1_bytes);
     if (a1 < 0) { give_up(a1); return; }
     int32_t* cand = reinterpret_cast<int32_t*>(spool + a1); float* dlp = reinterpret_cast<float*>(spool + a1 + (((long long)n_cand * 4 + 31) & ~31LL));
     // ---- 1b. expand + candidates before every container
-    {   int run = wbase;
-        for (int64_t gb = w0; gb < w1; gb += 4 * WS) {          // four groups per trip: their words are loaded together, then scanned one after the other
-            unsigned vv[4];
-            for (int u = 0; u < 4; u++) { const int64_t g = gb + u * WS, w = g + c.lane(); vv[u] = (g < w1 && sh.dirty[g >> 11] && w < w1) ? ws.bits[w] : 0u; }
-            for (int u = 0; u < 4; u++) {
-                const int64_t g0 = gb + u * WS; if (g0 >= w1) break;
-                if (!sh.dirty[g0 >> 11]) { if ((g0 & 2047) == 0 && c.lane() == 0) ws.cstart[g0 >> 11] = run; continue; }
-                const int64_t w = g0 + c.lane(); unsigned v = vv[u]; const int pc = popc(v); int incl = pc;
-                for (int d = 1; d < WS; d <<= 1) { int o = c.shfl(incl, c.lane() >= d ? c.lane() - d : 0); if (c.lane() >= d) incl += o; }
-                int o = run + incl - pc;
-                if (w < w1 && (w & 2047) == 0) ws.cstart[w >> 11] = o;
-                while (v) { int b = ffs32(v) - 1; v &= v - 1; cand[o++] = (int32_t)((w << 5) | b); }
-                run += c.shfl(incl, WS - 1);
-            }
-        }
-        if (c.tid() == 0) ws.cstart[ncont] = n_cand;
-    }
-    c.sync();
+    cand_expand(c, ix, ws, sh, sp, n_cand, cand);
     IFX_LTICK(0);   // count + expand
     // ---- 2. lengths, deleted flags (folded into the id), chunk table
     const bool any_deleted = ix.n_live != ix.n_docs;
@@ -261,10 +231,9 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
             c.sync();      // the window is rewritten for the next container
         }
     }
-    c.sync();
     IFX_LTICK(3);   // tf lookups
-    // ---- 4. bitset back to all-zero; record, queue, roofline accounting (SURVEY 8d)
-    clear_bits(nS == 0);
+    // ---- 4. bitset back to all-zero (when the LD1 unions were streamed, their container walk has zeroed the words); record, queue, roofline accounting (SURVEY 8d)
+    cand_clear(c, ix, ws, sh.dirty, nS > 0);
     IFX_LTICK(4);   // bitset cleared
     if (c.tid() == 0) {
         rec.off_cand = a1; rec.off_dl = a1 + (((long long)n_cand * 4 + 31) & ~31LL); rec.off_chunk = a2; rec.off_ctab = a2 + (long long)chunk_bytes;
@@ -282,7 +251,7 @@ IFX_FN void stage1_lookup(const Ctx& c, const DevIndex& ix, const QueryPlan& p, 
             algo += streamed ? full : (full < probe ? full : probe);
         }
         algo += 4ULL * (unsigned long long)n_cand;
-        atomic_add64(&bc->algo_bytes, algo); atomic_add64(&bc->s1_cand_sum, (unsigned long long)n_cand);
+        atomic_add64(&bc->algo_bytes, algo);
         if (out.dbg) { out.dbg[0] = n_cand; out.dbg[6] = forward ? 1 : 2; out.dbg[7] = n_chunks; out.dbg[8] = max_cnt; out.dbg[9] = Ta; }
     }
     c.sync();

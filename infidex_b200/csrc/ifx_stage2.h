@@ -129,11 +129,11 @@ IFX_FN void wm_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p, const
             if (up ? a > b : a < b) { sh.top_sorted[i] = b; sh.top_sorted[l] = a; uint16_t ra = sh.top_rank[i]; sh.top_rank[i] = sh.top_rank[l]; sh.top_rank[l] = ra; } } }
         c.sync();
     }
-    // ---- affix docs -> bitset (every touched word also in the summary bitset ws.bits2: one bit per word); membership of the top docs
+    // ---- affix docs -> candidate set (every touched word also in the summary ws.wm_sum: one bit per word); membership of the top docs
+    auto add = [&](int d) { cand_add(ws, sh.dirty, d); if (!((ws.wm_sum[d >> 10] >> ((d >> 5) & 31)) & 1u)) atomic_or(&ws.wm_sum[d >> 10], 1u << ((d >> 5) & 31)); };
     int any = 0;
     for (int a = 0; a < nw * 2; a++) { WmList L = sh.affix[a]; if (L.n > 0) any = 1;
-        for (int i = c.tid(); i < L.n; i += NT) { int d = L.p[i]; if (d < 0) continue;      // doc-id-range shards: the word's document lives on another shard
-            atomic_or(&ws.bits[d >> 5], 1u << (d & 31)); if (!((ws.bits2[d >> 10] >> ((d >> 5) & 31)) & 1u)) atomic_or(&ws.bits2[d >> 10], 1u << ((d >> 5) & 31)); sh.dirty[d >> 16] = 1; } }
+        for (int i = c.tid(); i < L.n; i += NT) { int d = L.p[i]; if (d >= 0) add(d); } }      // d < 0 (doc-id-range shards): the word's document lives on another shard
     if (c.tid() == 0) { int n = 0; for (int l = 0; l < n_lists; l++) if (sh.lists[l].n > 0) sh.nz[n++] = (uint16_t)l; sh.n_nz = n; }
     c.sync();
     const int nnz = sh.n_nz; if (nnz > 0) any = 1;
@@ -147,10 +147,10 @@ IFX_FN void wm_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p, const
     int my = 0; for (int k = c.tid(); k < nt; k += NT) my += sh.in_wm[k];
     const int n_overlap = block_sum(c, my, sh.scan);
     const int wm_limit = K - n_overlap > 0 ? K - n_overlap : 0;
-    // ---- leading elements of every list -> bitset (the first M elements of the union lie within the first M of each list)
+    // ---- leading elements of every list -> candidate set (the first M elements of the union lie within the first M of each list)
     const int M = K + nt + 2;
     for (int z = 0; z < nnz; z++) { WmList L = sh.lists[sh.nz[z]]; int m = L.n < M ? L.n : M;
-        for (int i = c.tid(); i < m; i += NT) { int d = L.p[i]; atomic_or(&ws.bits[d >> 5], 1u << (d & 31)); if (!((ws.bits2[d >> 10] >> ((d >> 5) & 31)) & 1u)) atomic_or(&ws.bits2[d >> 10], 1u << ((d >> 5) & 31)); sh.dirty[d >> 16] = 1; } }
+        for (int i = c.tid(); i < m; i += NT) add(L.p[i]); }
     c.sync();
     // ---- entries: (a) WM ∩ top ascending, base 0; the twin field holds the Stage-1 rank until group (c) is placed
     int ne = 0;
@@ -169,12 +169,12 @@ IFX_FN void wm_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p, const
             int64_t w0 = (int64_t)k * 2048, w1 = w0 + 2048; if (w1 > nwords) w1 = nwords;
             int per = (int)((w1 - w0 + NT - 1) / NT); int64_t my0 = w0 + (int64_t)c.tid() * per, my1 = my0 + per; if (my1 > w1) my1 = w1;
             int cnt = 0, live = 0;
-            for (int64_t w = my0; w < my1; w++) { if (!((ws.bits2[w >> 5] >> (w & 31)) & 1u)) continue;
+            for (int64_t w = my0; w < my1; w++) { if (!((ws.wm_sum[w >> 5] >> (w & 31)) & 1u)) continue;
                 unsigned v = ws.bits[w]; while (v) { int b = ffs32(v) - 1; v &= v - 1; int d = (int)((w << 5) | b); if (!ix.deleted[d]) live++; if (!sorted_contains(sh.top_sorted, nt, d)) cnt++; } }
             int tot; int off = block_excl_scan(c, cnt, sh.scan, tot);
             int ltot; int loff = block_excl_scan(c, live, sh.scan, ltot);
             int o = off, lo2 = loff;
-            for (int64_t w = my0; w < my1; w++) { if (!((ws.bits2[w >> 5] >> (w & 31)) & 1u)) continue;
+            for (int64_t w = my0; w < my1; w++) { if (!((ws.wm_sum[w >> 5] >> (w & 31)) & 1u)) continue;
                 unsigned v = ws.bits[w]; ws.bits[w] = 0;
                 while (v) { int b = ffs32(v) - 1; v &= v - 1; int d = (int)((w << 5) | b);
                     if (!ix.deleted[d]) { if (seen_live + lo2 < 2) sh.first_live[seen_live + lo2] = d; lo2++; }
@@ -182,12 +182,10 @@ IFX_FN void wm_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p, const
             int add = tot; if (taken + add > wm_limit) add = wm_limit - taken;
             taken += add; ne += add; seen_live += ltot;
             c.sync();                                              // every thread has read this container's summary words
-            for (int64_t sw = (w0 >> 5) + c.tid(); sw < ((w1 + 31) >> 5); sw += NT) ws.bits2[sw] = 0;
+            for (int64_t sw = (w0 >> 5) + c.tid(); sw < ((w1 + 31) >> 5); sw += NT) ws.wm_sum[sw] = 0;
         }
-        for (int64_t sw = (((int64_t)kdone * 2048) >> 5) + c.tid(); sw < nsum; sw += NT) { unsigned m = ws.bits2[sw]; if (!m) continue; ws.bits2[sw] = 0; while (m) { ws.bits[(sw << 5) | (ffs32(m) - 1)] = 0; m &= m - 1; } }
-        c.sync();
-        for (int k = c.tid(); k < ncont; k += NT) sh.dirty[k] = 0;
-        c.sync();
+        for (int64_t sw = (((int64_t)kdone * 2048) >> 5) + c.tid(); sw < nsum; sw += NT) { unsigned m = ws.wm_sum[sw]; if (!m) continue; ws.wm_sum[sw] = 0; while (m) { ws.bits[(sw << 5) | (ffs32(m) - 1)] = 0; m &= m - 1; } }
+        cand_clear(c, ix, ws, sh.dirty, true);
     }
     if (c.tid() == 0 && B.wm_cnt) { B.wm_cnt[q * 4 + 0] = n_overlap; B.wm_cnt[q * 4 + 1] = ne - n_overlap; B.wm_cnt[q * 4 + 2] = any; B.wm_cnt[q * 4 + 3] = n_overlap; }
     // ---- (c) every top candidate in rank order, base = score / top score; link twins with group (a)
