@@ -35,7 +35,7 @@ enum {
 /* per-query status bits in ifx_batch_result.status */
 enum {
     IFX_Q_OK = 0,
-    IFX_Q_UNSUPPORTED_OP = 2, /* MATCHES (regex) opcode; a query without a word of >= 3 characters on a doc-id-range SHARD (that path is built for the unsharded index) */
+    IFX_Q_UNSUPPORTED_OP = 2, /* MATCHES (regex) opcode; a query without a word of >= 3 characters over documents that share a DocumentKey */
     IFX_Q_OVERFLOW = 4,       /* a fixed device buffer was too small for this query */
     IFX_Q_EMPTY = 8           /* blank query -> empty result (SearchEngine.cs:295-296) */
 };
@@ -92,7 +92,7 @@ typedef struct ifx_index_image {
     int32_t n_champ_chars;            /* ShortQueryResolver champion lists of the 1-character prefixes: */
     const uint16_t* champ_chars;      /*   the character, */
     const int32_t* champ_off;         /*   [n_champ_chars + 1] */
-    const int32_t* champ_doc;         /*   internal doc ids, in the order BuildChampionLists leaves them (List.Sort by score descending, first 64) */
+    const int32_t* champ_doc;         /*   internal doc ids, in the order BuildChampionLists leaves them (List.Sort by score descending, first 64); a shard: the global lists, another shard's entries -1 */
     const float* champ_score;         /*   (precedence << 8) | base */
     int32_t n_raw;                    /* documents whose IndexedText differs from its normalised form (the short-query scorers read ToLowerInvariant(IndexedText)): */
     const int32_t* raw_doc;           /*   ascending internal ids, */
@@ -220,6 +220,19 @@ int  ifx_batch_stage1_restrict(ifx_batch* b, const uint8_t* keep /* [nq * depth]
 int  ifx_batch_wm_counts(ifx_batch* b, int32_t* buf /* [nq * 4] */);                 /* after phase 4 (WordMatcher lookups) */
 int  ifx_batch_wm_apply(ifx_batch* b, const int32_t* allowed /* [nq] */, const int32_t* any /* [nq] */);   /* then phase 5: coverage, fusion, finalize */
 int  ifx_batch_shard_info(ifx_batch* b, int32_t* info /* [nq * 8], HOST */, int64_t* dkey /* [nq * 2], HOST */);
+/* Short queries (no word of >= 3 characters) on shards, between phase 3 and ifx_batch_stage1_lists. ifx_batch_short_groups gives the number of
+ * groups (0: the batch holds no short query, nothing to do) and the group size G, the same on every shard; kind (HOST [nq], may be NULL):
+ * 0 not short, 1 one character, 2 several, | 4 when the <= 3-character rule of SearchPipeline applies. Then for every group g:
+ *   ifx_batch_short_step(b, 0, g, buf) -> all-reduce(sum) of buf -> step 1 -> all-reduce(max) of buf -> step 2
+ * buf: DEVICE int32[G] -- matched documents of each query of the group (ProcessFuzzyFallback below 100), then its largest integer score
+ * (BuildFinalScores normalises by it). Step 2 leaves the shard's exact Stage-1 list of every query of the group. */
+int  ifx_batch_short_groups(ifx_batch* b, int32_t* kind, int32_t* n_groups, int32_t* group_size);
+int  ifx_batch_short_step(ifx_batch* b, int step, int group, int32_t* buf);
+/* Then, after ifx_batch_wm_apply and before phase 5 (only when n_groups > 0): ifx_batch_short_hits(b, buf, 0) evaluates the coverage stage
+ * (phase 5 does not repeat it) and leaves each short query's largest coverage word hits on this shard in buf (DEVICE int32[nq]);
+ * all-reduce(max); ifx_batch_short_hits(b, buf, 1). A short query whose coverage found no word hit on any shard (and no WordMatcher
+ * document) falls back to its Stage-1 list on every shard, as SearchPipeline does. Steps out of order give IFX_ERR_INVALID. */
+int  ifx_batch_short_hits(ifx_batch* b, int32_t* buf, int set);
 
 /* Stage-1 only (Bm25Scorer.Search + ConsolidateSegments, src/Infidex/Indexing/Bm25Scorer.cs:56-193): row-major
  * [nq][depth] keys / scores, n[nq]. Used for intermediate parity checks and kernel-level measurement. */

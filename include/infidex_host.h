@@ -30,6 +30,10 @@ const uint8_t* ifx_builder_export_stats(ifx_builder* b, size_t* len);      /* va
 int ifx_builder_globalize(ifx_builder* b, int n_shards, int shard, const uint8_t* const* blobs);
 const float* ifx_builder_doc_lengths(ifx_builder* b, int* n);              /* after globalize: second exchange ... */
 int ifx_builder_set_global_lengths(ifx_builder* b, int n_shards, const float* const* lens, const int* counts);   /* ... avgdl over the whole corpus */
+/* champion lists of the one-character short queries over the whole corpus: export -> all-gather between the hosts (the size varies per
+ * shard) -> globalize. The image's champ_* arrays then hold the GLOBAL lists: entries of this shard as local ids, the others' as -1. */
+const uint8_t* ifx_builder_export_champions(ifx_builder* b, size_t* len);  /* valid until the next champion export on this thread */
+int ifx_builder_globalize_champions(ifx_builder* b, int n_shards, int shard, const uint8_t* const* blobs);
 
 /* SearchEngine.Search step 1 (src/Infidex/SearchEngine.cs:264-274): Trim + TextNormalizer.Normalize + ToLowerInvariant. Returns the output length. */
 int ifx_host_prepare_query(const uint16_t* in, int n, uint16_t* out, int cap);

@@ -202,6 +202,37 @@ void merge_records(std::vector<std::unique_ptr<KeyedRecords>>& parts, Csr& out, 
 
 struct FieldSpec { str name; int weight; int flags; };
 
+// ShortQueryResolver.BuildChampionLists: one character's candidates in ascending doc id order -> List.Sort by score descending
+using ChampCand = std::pair<uint16_t, int32_t>;      // (score, doc)
+void champ_sort(std::vector<ChampCand>& v) {
+    auto cmpf = [](const ChampCand& x, const ChampCand& y) { return y.first < x.first ? -1 : (y.first > x.first ? 1 : 0); };
+    DotnetIntroSort<ChampCand, decltype(cmpf)> srt{cmpf}; srt.sort(v.data(), (int)v.size());
+}
+
+// short-query structures (Indexing/ShortQuery/ShortQueryResolver.cs:83-160,268-311): per first character of a word of the index text `idx`,
+// (first token index, number of such word starts) -> precedence / base score against the document's lower-cased RAW title `raw`
+struct ChampRec { char16_t ch; uint16_t score; int32_t doc; };
+void champ_records(const str& raw, const str& idx, int d, str& tmp, std::vector<sv>& toks, std::vector<ChampRec>& out) {
+    tmp = raw; lower_inplace(tmp);                                // ToLowerInvariant(IndexedText), not normalised
+    // title tokens (split on the delimiters, empty entries removed) and trim
+    int n_tok = 0; toks.clear();
+    for (size_t i = 0; i < tmp.size();) { while (i < tmp.size() && is_delim(tmp[i])) i++; if (i >= tmp.size()) break; size_t s0 = i; while (i < tmp.size() && !is_delim(tmp[i])) i++; toks.emplace_back(tmp.data() + s0, i - s0); }
+    n_tok = (int)toks.size();
+    size_t tb = 0, te = tmp.size(); while (tb < te && is_ws(tmp[tb])) tb++; while (te > tb && is_ws(tmp[te - 1])) te--;
+    struct Acc { char16_t ch; int first_pos, n; }; Acc acc[64]; int na = 0; int ti = 0;
+    for (size_t i = 0; i < idx.size();) { while (i < idx.size() && is_delim(idx[i])) i++; if (i >= idx.size()) break; size_t s0 = i; while (i < idx.size() && !is_delim(idx[i])) i++;
+        const char16_t ch = idx[s0]; int a = 0; for (; a < na; a++) if (acc[a].ch == ch) break;
+        if (a == na) { if (na < 64) { acc[na].ch = ch; acc[na].first_pos = ti; acc[na].n = 1; na++; } } else acc[a].n++;
+        ti++; }
+    for (int a = 0; a < na; a++) {
+        const char16_t ch = acc[a].ch; int prec = 128; if (acc[a].first_pos == 0) prec |= 64;
+        bool any = false, first = false; for (int i = 0; i < n_tok; i++) if (toks[i].size() == 1 && toks[i][0] == ch) { any = true; if (i == 0) first = true; break; }
+        if (any) prec |= 32; if (first) prec |= 16; if (te - tb == 1 && tmp[tb] == ch) prec |= 8; if (n_tok <= 3) prec |= 32;
+        const int pos_c = 255 - std::min(acc[a].first_pos * 16, 240), dens = std::min(acc[a].n * 8, 32); const int base = std::max(0, std::min(255, pos_c + dens));
+        out.push_back({ch, (uint16_t)((prec << 8) | base), d});
+    }
+}
+
 str value_to_string(int kind, const void* col, const long long* offs, int d) {
     char buf[64];
     if (kind == 1) { const char16_t* b = (const char16_t*)col; return str(b + offs[d], (size_t)(offs[d + 1] - offs[d])); }
@@ -287,7 +318,7 @@ int ifx_builder_finish(ifx_builder* b, int threads) {
     struct Part {
         std::unique_ptr<KeyedRecords> terms, prefix, exact, ld1; Interner words; std::vector<int32_t> word_df; Interner affix; std::vector<int32_t> affix_last;
         std::vector<char16_t> text; std::vector<int64_t> text_len; std::vector<char16_t> ft; std::vector<uint32_t> ft_len; std::vector<uint16_t> tokc;
-        struct Champ { char16_t ch; uint16_t score; int32_t doc; }; std::vector<Champ> champs;      // ShortQueryResolver: one record per (first character of a word, document)
+        std::vector<ChampRec> champs;      // ShortQueryResolver: one record per (first character of a word, document)
         std::vector<int32_t> raw_doc; std::vector<char16_t> raw_chars; std::vector<int64_t> raw_len;   // documents whose raw IndexedText differs from its normalised form
     };
     std::vector<Part> parts(threads);
@@ -316,25 +347,8 @@ int ifx_builder_finish(ifx_builder* b, int threads) {
                 size_t ml = std::min<size_t>(3, i - s); for (size_t l = 1; l <= ml; l++) P.prefix->add_doc(P.prefix->key(sv(idx.data() + s, l)), d); }
             // short-query structures (Indexing/ShortQuery/ShortQueryResolver.cs:83-160,268-311): per first character of a word of the index text,
             // (first token index, number of such word starts) -> precedence / base score against the document's lower-cased RAW title
-            {   tmp = raw; lower_inplace(tmp);                                // ToLowerInvariant(IndexedText), not normalised
-                if (nrm != raw) { P.raw_doc.push_back(d); P.raw_chars.insert(P.raw_chars.end(), raw.begin(), raw.end()); P.raw_len.push_back((int64_t)raw.size()); }
-                // title tokens (split on the delimiters, empty entries removed) and trim
-                int n_tok = 0; sv first_tok; std::vector<sv>& toks = tok_scratch; toks.clear();
-                for (size_t i = 0; i < tmp.size();) { while (i < tmp.size() && is_delim(tmp[i])) i++; if (i >= tmp.size()) break; size_t s0 = i; while (i < tmp.size() && !is_delim(tmp[i])) i++; toks.emplace_back(tmp.data() + s0, i - s0); }
-                n_tok = (int)toks.size(); if (n_tok) first_tok = toks[0];
-                size_t tb = 0, te = tmp.size(); while (tb < te && is_ws(tmp[tb])) tb++; while (te > tb && is_ws(tmp[te - 1])) te--;
-                struct Acc { char16_t ch; int first_pos, n; }; Acc acc[64]; int na = 0; int ti = 0;
-                for (size_t i = 0; i < idx.size();) { while (i < idx.size() && is_delim(idx[i])) i++; if (i >= idx.size()) break; size_t s0 = i; while (i < idx.size() && !is_delim(idx[i])) i++;
-                    const char16_t ch = idx[s0]; int a = 0; for (; a < na; a++) if (acc[a].ch == ch) break;
-                    if (a == na) { if (na < 64) { acc[na].ch = ch; acc[na].first_pos = ti; acc[na].n = 1; na++; } } else acc[a].n++;
-                    ti++; }
-                for (int a = 0; a < na; a++) {
-                    const char16_t ch = acc[a].ch; int prec = 128; if (acc[a].first_pos == 0) prec |= 64;
-                    bool any = false, first = false; for (int i = 0; i < n_tok; i++) if (toks[i].size() == 1 && toks[i][0] == ch) { any = true; if (i == 0) first = true; break; }
-                    if (any) prec |= 32; if (first) prec |= 16; if (te - tb == 1 && tmp[tb] == ch) prec |= 8; if (n_tok <= 3) prec |= 32;
-                    const int pos_c = 255 - std::min(acc[a].first_pos * 16, 240), dens = std::min(acc[a].n * 8, 32); const int base = std::max(0, std::min(255, pos_c + dens));
-                    P.champs.push_back({ch, (uint16_t)((prec << 8) | base), d});
-                }
+            {   if (nrm != raw) { P.raw_doc.push_back(d); P.raw_chars.insert(P.raw_chars.end(), raw.begin(), raw.end()); P.raw_len.push_back((int64_t)raw.size()); }
+                champ_records(raw, idx, d, tmp, tok_scratch, P.champs);
             }
             // WordMatcher.Load / word-idf / metadata work on normalize(lower(IndexedText)); with a map the metadata on its CanonicalizeText
             // (VectorModel.cs:268-281), WordMatcher and word idf on the text as it is (SearchEngine.cs:143, VectorModel.cs:864-908)
@@ -376,8 +390,7 @@ int ifx_builder_finish(ifx_builder* b, int threads) {
             for (auto& P : parts) for (auto& cr : P.champs) by_ch[cr.ch].emplace_back(cr.score, cr.doc);
             b->champ_off.assign(1, 0);
             for (int ch = 0; ch < 65536; ch++) { auto& v = by_ch[ch]; if (v.empty()) continue;
-                auto cmpf = [](const std::pair<uint16_t, int32_t>& x, const std::pair<uint16_t, int32_t>& y) { return y.first < x.first ? -1 : (y.first > x.first ? 1 : 0); };
-                DotnetIntroSort<std::pair<uint16_t, int32_t>, decltype(cmpf)> srt{cmpf}; srt.sort(v.data(), (int)v.size());
+                champ_sort(v);
                 const size_t keep = std::min<size_t>(v.size(), 64);
                 b->champ_chars.push_back((uint16_t)ch); for (size_t i = 0; i < keep; i++) { b->champ_doc.push_back(v[i].second); b->champ_score.push_back((float)v[i].first); } b->champ_off.push_back((int32_t)b->champ_doc.size()); }
             if (b->champ_chars.empty()) b->champ_chars.push_back(0); if (b->champ_doc.empty()) { b->champ_doc.push_back(0); b->champ_score.push_back(0.f); }
@@ -566,6 +579,61 @@ int ifx_builder_globalize(ifx_builder* b, int n_shards, int shard, const uint8_t
     return IFX_OK;
 }
 
+// Champion lists of a shard (ShortQueryResolver.BuildChampionLists over the whole corpus). The export carries, per first character, every
+// candidate of this shard as (u16 score, local doc) in ascending doc order -- recomputed from the image's texts, so a builder keeps nothing
+// for it. Blob: int32 n_docs, int32 n_chars, then per character: u16 ch, int32 count, count x (u16 score, int32 doc).
+const uint8_t* ifx_builder_export_champions(ifx_builder* b, size_t* len) {
+    static thread_local Blob out; out.d.clear();
+    if (!b || !b->finished || !len) return nullptr;
+    const int N = (int)b->keys.size(); const int threads = (int)std::max(1u, std::min(std::thread::hardware_concurrency(), 64u));
+    const int nt = (int)std::max<int64_t>(1, std::min<int64_t>(threads, N / 4096 + 1));
+    std::vector<std::vector<ChampRec>> recs(nt);
+    par_for(N, nt, [&](int64_t d0, int64_t d1, int t) {
+        str raw, nrm, idx, meta, tmp; std::vector<sv> toks;
+        int64_t ri = std::lower_bound(b->raw_doc.begin(), b->raw_doc.begin() + (b->raw_off.size() - 1), (int32_t)d0) - b->raw_doc.begin();
+        for (int64_t d = d0; d < d1; d++) {
+            nrm.assign(b->text.data() + b->text_off[d], (size_t)(b->text_off[d + 1] - b->text_off[d]));
+            if (ri + 1 < (int64_t)b->raw_off.size() && b->raw_doc[ri] == (int32_t)d) { raw.assign(b->raw_chars.data() + b->raw_off[ri], (size_t)(b->raw_off[ri + 1] - b->raw_off[ri])); ri++; }
+            else raw = nrm;
+            idx = nrm; lower_inplace(idx);
+            if (b->has_syn()) { canon_into(idx, meta, b->syn); idx.swap(meta); }
+            champ_records(raw, idx, (int)d, tmp, toks, recs[t]);
+        } });
+    std::vector<int32_t> cnt(65536, 0); for (auto& r : recs) for (auto& c : r) cnt[c.ch]++;
+    std::vector<int64_t> at(65537, 0); for (int ch = 0; ch < 65536; ch++) at[ch + 1] = at[ch] + cnt[ch];
+    std::vector<ChampCand> flat((size_t)at[65536]); { std::vector<int64_t> pos(at.begin(), at.end() - 1); for (auto& r : recs) for (auto& c : r) flat[pos[c.ch]++] = {c.score, c.doc}; }
+    int nch = 0; for (int ch = 0; ch < 65536; ch++) if (cnt[ch]) nch++;
+    out.put<int32_t>(N); out.put<int32_t>(nch);
+    for (int ch = 0; ch < 65536; ch++) { if (!cnt[ch]) continue; out.put<uint16_t>((uint16_t)ch); out.put<int32_t>(cnt[ch]);
+        for (int64_t i = at[ch]; i < at[ch + 1]; i++) { out.put<uint16_t>(flat[i].first); out.put<int32_t>(flat[i].second); } }
+    *len = out.d.size(); return out.d.data();
+}
+
+// blobs[s] = ifx_builder_export_champions of shard s (all shards, in doc-range order). Replaces this builder's champion lists with the global
+// ones: per character the shards' candidates concatenated in shard order (= ascending global id), the same unstable sort, the first 64.
+// An entry this shard owns keeps its LOCAL id, another shard's is -1 (as affix_last_doc); the list length stays the global one.
+int ifx_builder_globalize_champions(ifx_builder* b, int n_shards, int shard, const uint8_t* const* blobs) {
+    if (!b || !b->finished || !blobs || n_shards < 1 || shard < 0 || shard >= n_shards) return IFX_ERR_INVALID;
+    std::vector<std::vector<ChampCand>> by_ch(65536); int64_t base = 0, doc_base = 0; int n_mine = 0;
+    for (int s = 0; s < n_shards; s++) {
+        Rd r{blobs[s]}; const int n = r.get<int32_t>(), nch = r.get<int32_t>();
+        if (s == shard) { doc_base = base; n_mine = n; }
+        for (int k = 0; k < nch; k++) { const uint16_t ch = r.get<uint16_t>(); const int c = r.get<int32_t>(); auto& v = by_ch[ch];
+            for (int i = 0; i < c; i++) { const uint16_t sc = r.get<uint16_t>(); const int32_t d = r.get<int32_t>(); v.emplace_back(sc, (int32_t)(base + d)); } }
+        base += n;
+    }
+    if (base > 0x7fffffffLL || n_mine != (int)b->keys.size()) return IFX_ERR_INVALID;
+    b->champ_chars.clear(); b->champ_doc.clear(); b->champ_score.clear(); b->champ_off.assign(1, 0);
+    for (int ch = 0; ch < 65536; ch++) { auto& v = by_ch[ch]; if (v.empty()) continue;
+        champ_sort(v); const size_t keep = std::min<size_t>(v.size(), 64);
+        b->champ_chars.push_back((uint16_t)ch);
+        for (size_t i = 0; i < keep; i++) { const int64_t l = v[i].second - doc_base; b->champ_doc.push_back(l >= 0 && l < n_mine ? (int32_t)l : -1); b->champ_score.push_back((float)v[i].first); }
+        b->champ_off.push_back((int32_t)b->champ_doc.size()); }
+    if (b->champ_chars.empty()) b->champ_chars.push_back(0); if (b->champ_doc.empty()) { b->champ_doc.push_back(0); b->champ_score.push_back(0.f); }
+    ifx_index_image& I = b->img;
+    I.n_champ_chars = (int)b->champ_off.size() - 1; I.champ_chars = b->champ_chars.data(); I.champ_off = b->champ_off.data(); I.champ_doc = b->champ_doc.data(); I.champ_score = b->champ_score.data();
+    return IFX_OK;
+}
 
 }  // extern "C"
 

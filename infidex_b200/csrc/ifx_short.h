@@ -160,13 +160,18 @@ IFX_FN void sq_topk_stage2(const Ctx& c, SqScratch S, SqTopShared& sh, int nblk,
     if (c.tid() == 0) { out_n[0] = n; out_total[0] = total; }
     c.sync();
 }
-// champion path (one character, max_results <= 64, list long enough): TopKHeap(max) over the first `max` champions, consolidated order
+// champion path (one character, max_results <= 64, list long enough): TopKHeap(max) over the first `max` champions, consolidated order.
+// On a doc-id-range shard the lists are the global ones and another shard's entries are -1: only this shard's entries among the first `max`
+// are written (the hosts' global cut merges them).
 IFX_FN void sq_champions(const Ctx& c, const DevIndex& ix, SqTopShared& sh, int ci, int m, int64_t* out_key, int32_t* out_doc, float* out_score, int32_t* out_n, int32_t* out_total) {
     sq_clear(c, sh, 0, 128); const int b = ix.champ_off[ci];
-    for (int i = c.tid(); i < m; i += c.nthreads()) { const int d = ix.champ_doc[b + i]; sh.score[i] = ix.champ_score[b + i]; sh.doc[i] = d; sh.key[i] = ix.doc_key[d]; }
-    c.sync(); sq_sort_desc(c, sh, 128);
-    for (int i = c.tid(); i < m; i += c.nthreads()) { out_key[i] = sh.key[i]; out_doc[i] = sh.doc[i]; out_score[i] = sh.score[i]; }
-    if (c.tid() == 0) { out_n[0] = m; out_total[0] = m; }
+    for (int i = c.tid(); i < m; i += c.nthreads()) { const int d = ix.champ_doc[b + i]; if (d < 0) continue; sh.score[i] = ix.champ_score[b + i]; sh.doc[i] = d; sh.key[i] = ix.doc_key[d]; }
+    c.sync();
+    if (c.tid() == 0) { int own = 0; for (int i = 0; i < m; i++) own += ix.champ_doc[b + i] >= 0; sh.bcast[0] = own; }
+    sq_sort_desc(c, sh, 128);
+    const int own = sh.bcast[0];
+    for (int i = c.tid(); i < own; i += c.nthreads()) { out_key[i] = sh.key[i]; out_doc[i] = sh.doc[i]; out_score[i] = sh.score[i]; }
+    if (c.tid() == 0) { out_n[0] = own; out_total[0] = own; }
     c.sync();
 }
 

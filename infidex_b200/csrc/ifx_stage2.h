@@ -28,6 +28,8 @@ struct Stage2Buffers {
     int32_t* wm_cnt;      // [nq][4] per shard: top docs that are also WordMatcher docs, WordMatcher-only entries taken, union non-empty, index of the first such entry
     const int32_t* g_di;  // doc-id-range shards: [nq][2] local id of the document at global Stage-1 rank 0 / 1 (-1: another shard's, -2: fewer than two ranks exist)
     const int32_t* s1_total;   // [nq] short-query path: documents matched by Stage 1 (the list itself is cut to the depth); null / 0 otherwise
+    const int32_t* s1_nglob;   // doc-id-range shards: [nq] Stage-1 list length over ALL shards (the mode decision of short queries); null otherwise
+    const int32_t* g_hits;     // doc-id-range shards: [nq] max coverage word hits over ALL shards of each short query (its fallback decision); null otherwise
     const float* gmax;    // doc-id-range shards: top Stage-1 score over ALL shards per query (normBm25, SearchPipeline.cs:411-413); null: the local list's first
     int32_t ent_cap;
 };
@@ -68,6 +70,7 @@ IFX_FN void wm_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p, const
     int32_t* e_doc = B.ent_doc + (size_t)q * cap; float* e_base = B.ent_base + (size_t)q * cap; int32_t* e_twin = B.ent_twin + (size_t)q * cap;
     if (c.tid() == 0) {
         int mode = 0; int n1 = n1_in < 0 ? 0 : n1_in;
+        if (p.short_kind != 0 && B.s1_nglob) n1 = B.s1_nglob[q];                     // a short query's list is a corpus-level quantity (a shard's n-gram queries keep the local count)
         if (p.status != 0) mode = 1;
         else if (p.is_short3 && n1 >= p.max_results) mode = 2;                       // SearchPipeline.cs:114-120
         else if (!p.enable_coverage || p.short_skip_coverage || p.short_no_cov) mode = 1;              // SearchPipeline.cs:157-170
@@ -472,8 +475,11 @@ IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p,
         }
         if (c.tid() == 0) {
             int result = nk;
-            if (O.shard_info) { if (result > p.max_results) result = p.max_results; }
-            else if (max_hits == 0 && !B.wm_any[q]) result = -1;                 // SearchPipeline.cs:418-419 -> coverage returned []
+            // SearchPipeline.cs:418-419: coverage returned [] -> the Stage-1 list. On shards a short query decides it on the word hits and the
+            // WordMatcher flag of ALL shards (g_hits, wm_any), so every shard takes the same branch; an n-gram query keeps the coverage records.
+            const bool none = (O.shard_info ? (p.short_kind != 0 && B.g_hits && B.g_hits[q] == 0) : max_hits == 0) && !B.wm_any[q];
+            if (none) result = -1;
+            else if (O.shard_info) { if (result > p.max_results) result = p.max_results; }
             else if (nk > 0) {
                 const int trunc = sh.bcast[4];
                 int count = trunc == -1 ? p.max_results : (trunc + 1 < p.max_results ? trunc + 1 : p.max_results);
@@ -483,11 +489,15 @@ IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p,
         }
         c.sync();
         n_rec = sh.n_keep;
-        if (n_rec < 0) { if (n1 > 0) mode = 1; else n_rec = 0; }              // SearchPipeline.cs:184-197 fallback to the TF-IDF backbone
+        if (n_rec < 0) { if (n1 > 0 || O.shard_info) mode = 1; else n_rec = 0; }      // SearchPipeline.cs:184-197 fallback to the TF-IDF backbone (a shard: whatever part of it is here)
     }
     if (mode != 0) {
         n_rec = mode == 2 ? (n1 < p.max_results ? n1 : p.max_results) : n1;
         if (n_rec > MAX_K) n_rec = MAX_K;
+        if (O.shard_info && p.short_kind != 0 && c.tid() == 0) {      // shards: no truncation facts; inf[6] = -1 tells the hosts the records are the Stage-1
+            int32_t* inf = O.shard_info + (size_t)q * 8;               // list, so TotalCandidates is the sum of the shards' totals
+            inf[0] = 0; inf[1] = 0; inf[2] = -1; inf[3] = -1; inf[4] = -1; inf[5] = -1; inf[6] = -1; inf[7] = 0; O.shard_dkey[q * 2] = -1; O.shard_dkey[q * 2 + 1] = -1;
+        }
         for (int i = c.tid(); i < n_rec; i += NT) { sh.keep_doc[i] = s1_doc[i]; sh.keep_score[i] = s1_score[i]; sh.keep_tie[i] = 0; }
         c.sync();
     }

@@ -3,8 +3,13 @@
 Layout (SURVEY.md 8e, DESIGN.md "multi-GPU"): rank r indexes the contiguous document range [r*N/R, (r+1)*N/R) rounded to multiples of
 65 536 (the reference's container size, so no 4096-chunk of Bm25Scorer is ever split). The statistics the search path reads as global
 quantities -- term ordinals, df / idf, N, avgdl, word idf, prefix-set cardinalities, the affix dictionary -- are exchanged once at build
-time (ifx_builder_export_stats -> all_gather -> ifx_builder_globalize). Every batch then runs on every shard, with three exchanges:
+time (ifx_builder_export_stats -> all_gather -> ifx_builder_globalize), and so are the champion lists of the one-character queries
+(ifx_builder_export_champions -> all_gather -> ifx_builder_globalize_champions). Every batch then runs on every shard, with these exchanges:
     all-reduce(sum)  document frequency of every LD1 union (its idf is a corpus-level quantity)                 16 int32 per query
+    all-reduce(sum)  the selector's cardinalities                                                               40 int32 per query
+    all-reduce(sum)  matched documents of every short query (only when the batch holds one)                     1 int32 per short query
+    all-reduce(max)  largest integer score of every short query (BuildFinalScores)                              1 int32 per short query
+    all-reduce(max)  largest coverage word hits per query (only with short queries: their fallback to Stage 1)   1 int32 per query
     all-gather       per-shard Stage-1 top-`depth` (key, score): global cut + global top score (normBm25)      depth * 12 B per query and shard
     all-gather       per-shard final records (key, score, tie, counts, facet rows): merged identically on every rank
 What is NOT exchanged (counted, never hidden -- `parity` in the bench line is the number of sampled queries whose merged records differ
@@ -70,13 +75,7 @@ class ShardedSearchEngine:
         eng._host.ifx_builder_export_stats.restype = C.c_void_p
         p = eng._host.ifx_builder_export_stats(C.c_void_p(eng._builder), C.byref(n))
         mine = np.ctypeslib.as_array((C.c_uint8 * n.value).from_address(p)).copy()
-        sizes = [torch.zeros(1, dtype=torch.int64, device=self.dev) for _ in range(self.world)]
-        dist.all_gather(sizes, torch.tensor([len(mine)], dtype=torch.int64, device=self.dev))
-        sizes = [int(s.item()) for s in sizes]; cap = max(sizes)
-        pad = np.zeros(cap, np.uint8); pad[: len(mine)] = mine
-        bufs = [torch.empty(cap, dtype=torch.uint8, device=self.dev) for _ in range(self.world)]
-        dist.all_gather(bufs, torch.from_numpy(pad).to(self.dev))
-        blobs = [b.cpu().numpy()[: sizes[i]].copy() for i, b in enumerate(bufs)]
+        blobs = self._all_gather_blob(mine)
         arr = (C.c_void_p * self.world)(*[bl.ctypes.data for bl in blobs])
         rc = eng._host.ifx_builder_globalize(C.c_void_p(eng._builder), self.world, self.rank, arr)
         if rc:
@@ -93,7 +92,26 @@ class ShardedSearchEngine:
         lens = [np.ascontiguousarray(x.cpu().numpy()[: nsz[i]]) for i, x in enumerate(lb)]
         larr = (C.c_void_p * self.world)(*[x.ctypes.data for x in lens]); carr = (C.c_int * self.world)(*nsz)
         eng._host.ifx_builder_set_global_lengths(C.c_void_p(eng._builder), self.world, larr, carr)
+        # third exchange: the champion lists of the one-character queries (every shard's candidates per first character -> the global lists)
+        eng._host.ifx_builder_export_champions.restype = C.c_void_p
+        cp = eng._host.ifx_builder_export_champions(C.c_void_p(eng._builder), C.byref(n))
+        cblobs = self._all_gather_blob(np.ctypeslib.as_array((C.c_uint8 * n.value).from_address(cp)).copy())
+        carr = (C.c_void_p * self.world)(*[bl.ctypes.data for bl in cblobs])
+        rc = eng._host.ifx_builder_globalize_champions(C.c_void_p(eng._builder), self.world, self.rank, carr)
+        if rc:
+            raise E.NativeError("ifx_builder_globalize_champions failed (%d)" % rc)
         eng._upload(eng._host.ifx_builder_image(C.c_void_p(eng._builder)))
+
+    def _all_gather_blob(self, mine):
+        """Every rank's byte blob (sizes differ): the sizes, then one all-gather padded to the largest."""
+        torch, dist = self.torch, self.dist
+        sizes = [torch.zeros(1, dtype=torch.int64, device=self.dev) for _ in range(self.world)]
+        dist.all_gather(sizes, torch.tensor([len(mine)], dtype=torch.int64, device=self.dev))
+        sizes = [int(s.item()) for s in sizes]; cap = max(sizes)
+        pad = np.zeros(cap, np.uint8); pad[: len(mine)] = mine
+        bufs = [torch.empty(cap, dtype=torch.uint8, device=self.dev) for _ in range(self.world)]
+        dist.all_gather(bufs, torch.from_numpy(pad).to(self.dev))
+        return [b.cpu().numpy()[: sizes[i]].copy() for i, b in enumerate(bufs)]
 
     # ---- search ------------------------------------------------------------------------------------------------------------------------
     def UploadBatch(self, queries):
@@ -152,13 +170,20 @@ class ShardedSearchEngine:
             eng._check(g.ifx_batch_select_counts(h, C.c_void_p(sc.data_ptr()), 1), "select counts set"); sync()
             self.exchange_ms["select_counts"] = self.exchange_ms.get("select_counts", 0.0) + 1e3 * (time.perf_counter() - t0)
             tp = time.perf_counter(); eng._check(g.ifx_batch_run_phase(h, 3, C.byref(st)), "phase 3"); self._acc("phase3", tp)
+            kind = self._short_queries(h, nq)
             t0 = time.perf_counter()
             key = torch.zeros(nq * K, dtype=torch.int64, device=self.dev); score = torch.zeros(nq * K, dtype=torch.float32, device=self.dev); n = torch.zeros(nq, dtype=torch.int32, device=self.dev)
             eng._check(g.ifx_batch_stage1_lists(h, C.c_void_p(key.data_ptr()), C.c_void_p(score.data_ptr()), C.c_void_p(n.data_ptr())), "stage1 lists")
             W = self.world
             ks = [torch.empty_like(key) for _ in range(W)]; ss = [torch.empty_like(score) for _ in range(W)]; ns = [torch.empty_like(n) for _ in range(W)]
             dist.all_gather(ks, key); dist.all_gather(ss, score); dist.all_gather(ns, n)
-            keep, gmax, nglob = self._global_cut(ks, ss, ns, nq, K)
+            self.last_s1_counts = ns          # every shard's Stage-1 list lengths of the last batch ([W] tensors of [nq]; diagnostics, tests)
+            lim = None
+            if kind is not None:      # a short query's list is cut where the unsharded one is: at max_results when it is one character or is_short3
+                mx = torch.tensor([q.MaxNumberOfRecordsToReturn for q in queries], dtype=torch.int64, device=self.dev).clamp(max=K)
+                kd = torch.from_numpy(kind).to(self.dev)
+                lim = torch.where(((kd & 3) == 1) | ((kd & 4) != 0), mx, torch.full_like(mx, K))
+            keep, gmax, nglob = self._global_cut(ks, ss, ns, nq, K, lim)
             self._keep, self._gmax = keep, gmax          # borrowed by the library until the last phase has run
             eng._check(g.ifx_batch_stage1_restrict(h, C.c_void_p(keep.data_ptr()), C.c_void_p(gmax.data_ptr()), C.c_void_p(nglob.data_ptr())), "stage1 restrict"); sync()
             self.exchange_ms["stage1"] += 1e3 * (time.perf_counter() - t0)
@@ -175,6 +200,12 @@ class ShardedSearchEngine:
             anyg = (WC[:, :, 2].sum(1) > 0).to(torch.int32).contiguous()
             eng._check(g.ifx_batch_wm_apply(h, C.c_void_p(allowed.data_ptr()), C.c_void_p(anyg.data_ptr())), "wm apply"); sync()
             self.exchange_ms["wm"] = self.exchange_ms.get("wm", 0.0) + 1e3 * (time.perf_counter() - t0)
+            if kind is not None:      # short queries: coverage word hits over all shards decide the fallback to the Stage-1 list on every shard alike
+                t0 = time.perf_counter(); hits = torch.zeros(nq, dtype=torch.int32, device=self.dev)
+                eng._check(g.ifx_batch_short_hits(h, C.c_void_p(hits.data_ptr()), 0), "short hits get")
+                dist.all_reduce(hits, op=dist.ReduceOp.MAX)
+                eng._check(g.ifx_batch_short_hits(h, C.c_void_p(hits.data_ptr()), 1), "short hits set"); sync()
+                self.exchange_ms["short"] = self.exchange_ms.get("short", 0.0) + 1e3 * (time.perf_counter() - t0)
             tp = time.perf_counter(); eng._check(g.ifx_batch_run_phase(h, 5, C.byref(st)), "phase 5"); self._acc("phase5", tp)
             tp = time.perf_counter(); eng._check(g.ifx_batch_download(h, C.byref(packed["out"])), "ifx_batch_download")
             info = np.zeros((nq, 8), np.int32); dkey = np.zeros((nq, 2), np.int64)
@@ -185,18 +216,38 @@ class ShardedSearchEngine:
                 g.ifx_batch_free(h); self._cached_h = None
             raise
         t0 = time.perf_counter()
-        merged = self._merge(queries, packed["bufs"], cap)
+        merged = self._merge(queries, packed["bufs"], cap, kind)
         self.exchange_ms["final"] += 1e3 * (time.perf_counter() - t0)
         return merged if raw else self._results(queries, merged)
+
+    def _short_queries(self, h, nq):
+        """The short queries of the batch (no word of >= 3 characters), group by group: matched documents summed over the shards (fuzzy
+        fallback below 100), then the largest integer score (BuildFinalScores). Returns the per-query kinds, or None when there is none --
+        the device counts them from the texts, so every rank takes the same branch."""
+        import time
+        eng, torch, dist, g = self.eng, self.torch, self.dist, self.eng._gpu
+        ng = C.c_int(0); gs = C.c_int(0); kind = np.zeros(nq, np.int32)
+        eng._check(g.ifx_batch_short_groups(h, E._p(kind), C.byref(ng), C.byref(gs)), "short groups")
+        if ng.value == 0:
+            return None
+        t0 = time.perf_counter()
+        buf = torch.zeros(gs.value, dtype=torch.int32, device=self.dev); ptr = C.c_void_p(buf.data_ptr())
+        for grp in range(ng.value):
+            eng._check(g.ifx_batch_short_step(h, 0, grp, ptr), "short step 0"); dist.all_reduce(buf)
+            eng._check(g.ifx_batch_short_step(h, 1, grp, ptr), "short step 1"); dist.all_reduce(buf, op=dist.ReduceOp.MAX)
+            eng._check(g.ifx_batch_short_step(h, 2, grp, ptr), "short step 2")
+        self.exchange_ms["short"] = self.exchange_ms.get("short", 0.0) + 1e3 * (time.perf_counter() - t0)
+        return kind
 
     def _acc(self, name, t0):
         import time
         self.host_ms[name] = self.host_ms.get(name, 0.0) + 1e3 * (time.perf_counter() - t0)
 
-    def _global_cut(self, ks, ss, ns, nq, K):
+    def _global_cut(self, ks, ss, ns, nq, K, lim=None):
         """Membership of this rank's Stage-1 entries in the global top-K by (score desc, key asc), and the global top score per query.
         Every shard's list is already in that order, so an entry's global rank is its local rank plus, per other shard, the number of
-        entries ahead of it -- W - 1 binary searches over packed (score bits, inverted key) words instead of a sort of all W * K entries."""
+        entries ahead of it -- W - 1 binary searches over packed (score bits, inverted key) words instead of a sort of all W * K entries.
+        `lim` ([nq], optional): a shorter global list for some queries (short queries cut at max_results)."""
         torch = self.torch; W = self.world; dev = ss[0].device
         N = torch.stack(ns, 1).clamp(min=0, max=K)                                             # [nq, W]
         slot = torch.arange(K, device=dev).view(1, K)
@@ -210,19 +261,19 @@ class ShardedSearchEngine:
             comp = (ss[r].view(nq, K).view(torch.int32).to(torch.int64) << 32) | (0xFFFFFFFF - k)      # larger = earlier in the list order
             negc.append(torch.where(v, -comp, torch.full_like(comp, big)).contiguous())           # ascending along the list; invalid slots last
         if not fits:
-            return self._global_cut_sort(ks, ss, ns, nq, K)
+            return self._global_cut_sort(ks, ss, ns, nq, K, lim)
         mine = negc[self.rank]; grank = slot.expand(nq, K).clone()
         for o in range(W):
             if o != self.rank:
                 grank += torch.searchsorted(negc[o], mine, right=False)
         valid = slot < N[:, self.rank].view(nq, 1)
-        keep = torch.where(valid & (grank < K), torch.where(grank == 0, 2, torch.where(grank == 1, 3, 1)), 0).to(torch.uint8).contiguous().view(-1)      # 2 / 3: global rank 0 / 1 (docIndex 0 / 1)
+        keep = torch.where(valid & (grank < (K if lim is None else lim.view(nq, 1))), torch.where(grank == 0, 2, torch.where(grank == 1, 3, 1)), 0).to(torch.uint8).contiguous().view(-1)      # 2 / 3: global rank 0 / 1 (docIndex 0 / 1)
         first = torch.stack([torch.where(N[:, r] > 0, ss[r].view(nq, K)[:, 0], torch.zeros((), dtype=ss[r].dtype, device=dev)) for r in range(W)], 1)
         gmax = first.max(dim=1).values.clamp(min=0).contiguous()
         nglob = N.sum(1).clamp(max=K).to(torch.int32).contiguous()
         return keep, gmax, nglob
 
-    def _global_cut_sort(self, ks, ss, ns, nq, K):
+    def _global_cut_sort(self, ks, ss, ns, nq, K, lim=None):
         """General form (keys beyond 32 bits): two stable sorts over all W * K entries."""
         torch = self.torch; W = self.world
         S = torch.stack([s.view(nq, K) for s in ss], 1).reshape(nq, W * K); Kk = torch.stack([k.view(nq, K) for k in ks], 1).reshape(nq, W * K)
@@ -234,6 +285,8 @@ class ShardedSearchEngine:
         i2 = torch.argsort(S1, dim=1, descending=True, stable=True)
         order = torch.gather(i1, 1, i2)[:, :K]                                                 # flat positions of the global top-K
         top_valid = torch.gather(valid, 1, order)
+        if lim is not None:
+            top_valid = top_valid & (torch.arange(K, device=S.device).view(1, K) < lim.view(nq, 1))
         mark = torch.zeros(nq, W * K, dtype=torch.uint8, device=S.device)
         flag = top_valid.to(torch.uint8); flag[:, 0] *= 2                                     # 2: global rank 0, 3: global rank 1 (docIndex 0 / 1)
         if K > 1:
@@ -244,7 +297,7 @@ class ShardedSearchEngine:
         nglob = valid.sum(1).clamp(max=K).to(torch.int32).contiguous()
         return keep, gmax, nglob
 
-    def _merge(self, queries, bufs, cap):
+    def _merge(self, queries, bufs, cap, kind=None):
         """All-gather of every shard's records; merged by ScoreEntry order (Score desc, Tiebreaker desc, DocumentId asc) and cut to max."""
         torch, dist, W = self.torch, self.dist, self.world
         import time
@@ -287,6 +340,11 @@ class ShardedSearchEngine:
             status_t |= M[:, r, 2]
         o_key = t_key.cpu().numpy(); o_score = t_sbits.to(torch.int32).cpu().numpy().view(np.float32); o_tie = t_tie.to(torch.uint8).cpu().numpy(); o_n = t_n.cpu().numpy()
         total = o_n.copy(); status = status_t.cpu().numpy(); self._acc("merge_sort_cut", tp)
+        self.last_shard_info = M[:, :, 4:12]          # every shard's truncation facts of the last batch ([nq, W, 8]; diagnostics, tests)
+        if kind is not None:      # a short query whose records are its Stage-1 list (shard_info[6] == -1): TotalCandidates counts the whole list
+            lst = (M[:, :, 10] == -1).cpu().numpy(); short = kind != 0
+            total = np.where(short & lst.any(1), M[:, :, 1].sum(1).cpu().numpy(), total)
+            status = np.where(short & lst.any(1) & ~lst.all(1), status | 2, status)      # shards that disagree on the answer's kind: flagged, never mixed
         self.last_raw = (o_key, o_score, o_tie, o_n, total, status)
         facets_all = None
         if any(q.EnableFacets for q in queries):          # facet rows travel as strings (value ids are per-shard dictionaries)
