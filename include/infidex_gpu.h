@@ -139,7 +139,8 @@ typedef struct ifx_query {
  *   boost_strength[i] (int)Boost[i].BoostStrength
  *   sort_column       column index (needs ifx_column_set_order first), IFX_SORT_NONE, or IFX_SORT_ALL_NULL for a SortBy field no
  *                     document has (every value null: the sort still runs and permutes equal values)
- * Records of a doc-id-range SHARD get IFX_Q_UNSUPPORTED_OP (post-processing belongs after the hosts' merge); a list the device holds only
+ * Records of a doc-id-range SHARD get IFX_Q_UNSUPPORTED_OP (post-processing belongs after the hosts' merge, which applies the filter and
+ * builds the facets but has no boosts or SortBy yet: see ifx_batch_shard_records); a list the device holds only
  * in part (the short-query path returns its whole list) gets IFX_Q_OVERFLOW instead of a sorted prefix. The blank query ignores both. */
 enum { IFX_MAX_BOOSTS = 16, IFX_SORT_NONE = -1, IFX_SORT_ALL_NULL = -2 };
 typedef struct ifx_query_post {
@@ -233,6 +234,24 @@ int  ifx_batch_short_step(ifx_batch* b, int step, int group, int32_t* buf);
  * all-reduce(max); ifx_batch_short_hits(b, buf, 1). A short query whose coverage found no word hit on any shard (and no WordMatcher
  * document) falls back to its Stage-1 list on every shard, as SearchPipeline does. Steps out of order give IFX_ERR_INVALID. */
 int  ifx_batch_short_hits(ifx_batch* b, int32_t* buf, int set);
+/* Filters and facets on shards. The hosts truncate the merged coverage records (CalculateTruncationIndex) and cut a list answered by the
+ * <= 3-character rule at max_results (shard_info[6] == 0 for both), and the filter runs after that, as in SearchEngine.Search. So a shard
+ * reports those records UNFILTERED, and ifx_batch_shard_records (after phase 5; out: DEVICE int32 [nq][cap][stride], stride = 1 + F, F =
+ * facetable columns, cap = the batch's max_results; another stride is IFX_ERR_INVALID) gives per record its filter outcome (1 pass / 0 fail,
+ * evaluated by the shard that owns the document) and the value id of each facetable column in column order (-1: null or empty).
+ * A query answered with its WHOLE Stage-1 list (shard_info[6] == -1: EnableCoverage off, a 3-character query over a prefix of > 500
+ * documents, a short query) keeps its filter on the shard: TotalCandidates is the sum of the shards' totals, and its facet rows (over the
+ * shard's filtered part of the list, no cut at 100 values per column, at most facet_cap rows: more sets IFX_Q_OVERFLOW) come with
+ * ifx_batch_download for the hosts to sum. The blank query with EnableFacets (shard_info[6] == -2): the shards' records in shard order, then
+ * Take(max). Value ids are the same on every shard once the columns were globalized (ifx_builder_globalize_columns).
+ * ifx_batch_set_facet_cap: facet rows per query of the batch's outputs (an uploaded batch starts with 0: no facet rows).
+ * ifx_batch_facet_table: the facet table of every query with enable_facets from rows = DEVICE int32 [nq][m][3] (column, value id, count;
+ * count 0 = no row), e.g. the records the hosts kept, one row per facetable column: counts summed per value id, ordered by count descending,
+ * then by value as FacetBuilder orders keys, the first 100 per column, at most facet_cap rows (more sets IFX_Q_OVERFLOW in status). Outputs:
+ * DEVICE [nq][facet_cap] column / value / count as in ifx_batch_result, n_facets [nq]; status [nq] is read and updated. */
+int  ifx_batch_shard_records(ifx_batch* b, int32_t* out, int32_t stride);
+int  ifx_batch_set_facet_cap(ifx_batch* b, int32_t facet_cap);
+int  ifx_batch_facet_table(ifx_batch* b, const int32_t* rows, int32_t m, int32_t* column, int32_t* value, int32_t* count, int32_t* n_facets, int32_t* status);
 
 /* Stage-1 only (Bm25Scorer.Search + ConsolidateSegments, src/Infidex/Indexing/Bm25Scorer.cs:56-193): row-major
  * [nq][depth] keys / scores, n[nq]. Used for intermediate parity checks and kernel-level measurement. */

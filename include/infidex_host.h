@@ -34,6 +34,11 @@ int ifx_builder_set_global_lengths(ifx_builder* b, int n_shards, const float* co
  * shard) -> globalize. The image's champ_* arrays then hold the GLOBAL lists: entries of this shard as local ids, the others' as -1. */
 const uint8_t* ifx_builder_export_champions(ifx_builder* b, size_t* len);  /* valid until the next champion export on this thread */
 int ifx_builder_globalize_champions(ifx_builder* b, int n_shards, int shard, const uint8_t* const* blobs);
+/* filter / facet / sort columns over the whole corpus: export -> all-gather between the hosts -> globalize. Afterwards every column's
+ * dictionary is the unsharded builder's (values in first-occurrence order over the shards in doc order), this shard's value ids index it,
+ * and the field's runtime kind is the corpus's (ifx_builder_column_order): a value id means the same on every shard. */
+const uint8_t* ifx_builder_export_columns(ifx_builder* b, size_t* len);    /* valid until the next column export on this thread */
+int ifx_builder_globalize_columns(ifx_builder* b, int n_shards, int shard, const uint8_t* const* blobs);
 
 /* SearchEngine.Search step 1 (src/Infidex/SearchEngine.cs:264-274): Trim + TextNormalizer.Normalize + ToLowerInvariant. Returns the output length. */
 int ifx_host_prepare_query(const uint16_t* in, int n, uint16_t* out, int cap);

@@ -635,6 +635,41 @@ int ifx_builder_globalize_champions(ifx_builder* b, int n_shards, int shard, con
     return IFX_OK;
 }
 
+// Filter / facet / sort columns of a shard: per column the field's runtime kind and the dictionary in first-occurrence order over this shard's
+// documents. Blob: int32 n_columns, then per column: int32 kind, strings.
+const uint8_t* ifx_builder_export_columns(ifx_builder* b, size_t* len) {
+    static thread_local Blob out; out.d.clear();
+    if (!b || !b->finished || !len) return nullptr;
+    out.put<int32_t>((int32_t)b->col_off.size());
+    for (size_t c = 0; c < b->col_off.size(); c++) { out.put<int32_t>(b->col_kind[c]); out.strings(b->col_chars[c].data(), b->col_off[c].data(), (int)b->col_off[c].size() - 1); }
+    *len = out.d.size(); return out.d.data();
+}
+
+// blobs[s] = ifx_builder_export_columns of shard s (all shards, in doc-range order). Every column's dictionary becomes the corpus's: the
+// values in first-occurrence order over the shards in doc order, which is the order the unsharded builder interns them in; this shard's value
+// ids are remapped to it, and the field's runtime kind is combined over the shards as ifx_builder_add_docs combines it over chunks.
+int ifx_builder_globalize_columns(ifx_builder* b, int n_shards, int shard, const uint8_t* const* blobs) {
+    if (!b || !b->finished || !blobs || n_shards < 1 || shard < 0 || shard >= n_shards) return IFX_ERR_INVALID;
+    const int NC = (int)b->col_off.size();
+    std::vector<Interner> g(NC); std::vector<int> kind(NC, 0); std::vector<std::vector<int32_t>> l2g(NC);
+    for (int s = 0; s < n_shards; s++) {
+        Rd r{blobs[s]}; if (r.get<int32_t>() != NC) return IFX_ERR_INVALID;
+        for (int c = 0; c < NC; c++) {
+            const int k = r.get<int32_t>(); const StrView v = rd_strings(r);
+            if (k != 0) kind[c] = (kind[c] == 0 || kind[c] == k) ? k : -1;
+            for (int i = 0; i < v.n; i++) { const int id = g[c].intern(v.at(i)); if (s == shard) l2g[c].push_back(id); }
+        }
+    }
+    for (int c = 0; c < NC; c++) {
+        if ((int)l2g[c].size() != (int)b->col_off[c].size() - 1) return IFX_ERR_INVALID;
+        for (auto& id : b->col_ids[c]) if (id >= 0) id = l2g[c][id];
+        b->col_chars[c].assign(g[c].arena.begin(), g[c].arena.end()); if (b->col_chars[c].empty()) b->col_chars[c].push_back(0);
+        b->col_off[c] = g[c].off; b->col_kind[c] = kind[c];
+        b->cols[c].dict = {(const uint16_t*)b->col_chars[c].data(), b->col_off[c].data(), (int)b->col_off[c].size() - 1};
+    }
+    return IFX_OK;
+}
+
 }  // extern "C"
 
 extern "C" void ifx_builder_destroy(ifx_builder* b) { for (size_t i = 0; i < g_shard_extra.size(); i++) if (g_shard_extra[i].first == b) { delete g_shard_extra[i].second; g_shard_extra.erase(g_shard_extra.begin() + i); break; } delete b; }

@@ -35,7 +35,8 @@ struct Stage2Buffers {
 };
 
 struct FinalOut { int64_t* key; float* score; uint8_t* tie; int32_t* n; int32_t* total; int32_t* status; int32_t* facet_col; int32_t* facet_val; int32_t* facet_cnt; int32_t* n_facets; int32_t cap, fcap;
-                  int32_t* shard_info; int64_t* shard_dkey; };     // doc-id-range shards (non-null): no local truncation, [nq][8] / [nq][2] facts for the hosts' merge
+                  int32_t* shard_info; int64_t* shard_dkey;      // doc-id-range shards (non-null): no local truncation, [nq][8] / [nq][2] facts for the hosts' merge
+                  int32_t* rec_post; int32_t rec_stride; };      // shards: [nq][cap][rec_stride] per record: filter pass, value id of every facetable column (-1 null / empty)
 
 struct WmList { const int32_t* p; int32_t n; };
 
@@ -70,7 +71,7 @@ IFX_FN void wm_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p, const
     int32_t* e_doc = B.ent_doc + (size_t)q * cap; float* e_base = B.ent_base + (size_t)q * cap; int32_t* e_twin = B.ent_twin + (size_t)q * cap;
     if (c.tid() == 0) {
         int mode = 0; int n1 = n1_in < 0 ? 0 : n1_in;
-        if (p.short_kind != 0 && B.s1_nglob) n1 = B.s1_nglob[q];                     // a short query's list is a corpus-level quantity (a shard's n-gram queries keep the local count)
+        if ((p.short_kind != 0 || p.is_short3) && B.s1_nglob) n1 = B.s1_nglob[q];    // shards: the <= 3-character rule reads the list length over ALL shards, so every shard takes the same mode
         if (p.status != 0) mode = 1;
         else if (p.is_short3 && n1 >= p.max_results) mode = 2;                       // SearchPipeline.cs:114-120
         else if (!p.enable_coverage || p.short_skip_coverage || p.short_no_cov) mode = 1;              // SearchPipeline.cs:157-170
@@ -387,6 +388,32 @@ IFX_FN void post_process(const Ctx& c, const DevIndex& ix, const ifx_query_post&
     c.sync();
 }
 
+// ---- FacetBuilder.BuildFacets over n items, one thread: per facetable column the value ids id_of(col, i) (< 0: none) with weight cnt_of(i) are
+// summed per id -- empty strings are not counted --, ordered by OrderByDescending(count).ThenBy(key) (a stable insertion sort; key order =
+// case-insensitive, then lower-case first, SURVEY Q12), and the first `per_col` of every column become rows (col, id, count) of `row`; rows
+// beyond `fcap` set IFX_Q_OVERFLOW in `status`. fv / fc: scratch of n entries. Returns the number of rows written.
+template <class IdOf, class CntOf>
+IFX_FN int facet_table(const DevIndex& ix, int n, IdOf id_of, CntOf cnt_of, int per_col, int32_t* fv, int32_t* fc,
+                       int32_t* row_col, int32_t* row_val, int32_t* row_cnt, int fcap, int& status) {
+    int nf = 0;
+    for (int col = 0; col < ix.n_columns; col++) {
+        const Column& C = ix.columns[col]; if (!(C.flags & 2)) continue;
+        int nu = 0;
+        for (int i = 0; i < n; i++) { const int id = id_of(col, i); const int w = cnt_of(i); if (id < 0 || w <= 0) continue; if (C.dict.off[id + 1] == C.dict.off[id]) continue;
+            int u = 0; for (; u < nu; u++) if (fv[u] == id) { fc[u] += w; break; } if (u == nu) { fv[nu] = id; fc[nu] = w; nu++; } }
+        for (int a = 1; a < nu; a++) { int v = fv[a], cn = fc[a]; int b = a - 1;
+            while (b >= 0) { bool gt;
+                if (fc[b] != cn) gt = fc[b] < cn;
+                else { Str x{C.dict.chars + C.dict.off[fv[b]], (int)(C.dict.off[fv[b] + 1] - C.dict.off[fv[b]])}, y{C.dict.chars + C.dict.off[v], (int)(C.dict.off[v + 1] - C.dict.off[v])};
+                    int cv = cmp_ic_str(ix, x, y); if (cv == 0) cv = -cmp_ordinal(x.p, x.n, y.p, y.n); gt = cv > 0; }
+                if (!gt) break; fv[b + 1] = fv[b]; fc[b + 1] = fc[b]; b--; }
+            fv[b + 1] = v; fc[b + 1] = cn; }
+        const int lim = nu < per_col ? nu : per_col;
+        for (int u = 0; u < lim; u++) { if (nf < fcap) { row_col[nf] = col; row_val[nf] = fv[u]; row_cnt[nf] = fc[u]; nf++; } else status |= 4; }
+    }
+    return nf;
+}
+
 // `post`: [nq] boosts / SortBy per query, or null (no post-processing: exactly the plain search)
 IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p, const int32_t* s1_doc, const float* s1_score, int n1,
                            const Stage2Buffers& B, const FilterProg* filters, int n_filters, const ifx_query_post* post, FinShared& sh, const FinalOut& O, int q) {
@@ -494,9 +521,9 @@ IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p,
     if (mode != 0) {
         n_rec = mode == 2 ? (n1 < p.max_results ? n1 : p.max_results) : n1;
         if (n_rec > MAX_K) n_rec = MAX_K;
-        if (O.shard_info && p.short_kind != 0 && c.tid() == 0) {      // shards: no truncation facts; inf[6] = -1 tells the hosts the records are the Stage-1
-            int32_t* inf = O.shard_info + (size_t)q * 8;               // list, so TotalCandidates is the sum of the shards' totals
-            inf[0] = 0; inf[1] = 0; inf[2] = -1; inf[3] = -1; inf[4] = -1; inf[5] = -1; inf[6] = -1; inf[7] = 0; O.shard_dkey[q * 2] = -1; O.shard_dkey[q * 2 + 1] = -1;
+        if (O.shard_info && c.tid() == 0) {      // shards: no truncation facts; inf[6] = -1 tells the hosts the records are the WHOLE Stage-1 list (filtered
+            int32_t* inf = O.shard_info + (size_t)q * 8;      // here; TotalCandidates and facet rows summed over the shards), 0 a list the hosts cut at max before they filter
+            inf[0] = 0; inf[1] = 0; inf[2] = -1; inf[3] = -1; inf[4] = -1; inf[5] = -1; inf[6] = (mode == 1 || p.short_kind != 0) ? -1 : 0; inf[7] = 0; O.shard_dkey[q * 2] = -1; O.shard_dkey[q * 2 + 1] = -1;
         }
         for (int i = c.tid(); i < n_rec; i += NT) { sh.keep_doc[i] = s1_doc[i]; sh.keep_score[i] = s1_score[i]; sh.keep_tie[i] = 0; }
         c.sync();
@@ -519,15 +546,20 @@ IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p,
         c.sync();
         if (sh.bcast[5]) status |= 2;
         n_rec = have < want ? have : want;
+        if (O.shard_info && c.tid() == 0) O.shard_info[(size_t)q * 8 + 6] = -2;      // shards: the hosts take the shards' records in shard order
     }
+    // Shards: the hosts truncate the merged coverage records (mode 0) and cut a list of the <= 3-character rule at max (mode 2), then filter:
+    // such a shard reports its records unfiltered, with their filter outcomes and facet value ids (O.rec_post). A whole Stage-1 list (mode 1;
+    // a short query's list in any mode: the global cut already kept it at max) is filtered here, and the blank query's browse above.
+    const bool host_filter = O.shard_info && !browse && !(mode == 1 || (mode != 0 && p.short_kind != 0));
     // ---- ApplyFilter (ResultProcessor.cs:56-69), ApplyBoosts / ApplySort, facets over the post-processed records, Take(max)
     if (c.tid() == 0) {
         int nk = n_rec; bool unsupported = false;
         if (browse) { /* filtered above */ }
         else if (p.filter_id >= 0 && p.filter_id < n_filters) {
             const FilterProg fp = filters[p.filter_id]; int w = 0;
-            for (int i = 0; i < nk; i++) if (filter_exec(ix, fp, sh.keep_doc[i], unsupported)) { sh.keep_doc[w] = sh.keep_doc[i]; sh.keep_score[w] = sh.keep_score[i]; sh.keep_tie[w] = sh.keep_tie[i]; w++; }
-            nk = w;
+            if (!host_filter) for (int i = 0; i < nk; i++) if (filter_exec(ix, fp, sh.keep_doc[i], unsupported)) { sh.keep_doc[w] = sh.keep_doc[i]; sh.keep_score[w] = sh.keep_score[i]; sh.keep_tie[w] = sh.keep_tie[i]; w++; }
+            if (!host_filter) nk = w;
         } else if (p.filter_id >= n_filters) status |= 2;
         if (unsupported) status |= 2;
         sh.bcast[5] = 0; sh.bcast[6] = nk; sh.bcast[7] = status;
@@ -544,28 +576,26 @@ IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p,
     if (c.tid() == 0) {
         int nk = sh.bcast[6];
         int nf = 0;
-        if (p.enable_facets && O.fcap > 0 && nk > 0) {
-            for (int col = 0; col < ix.n_columns; col++) {
-                const Column& C = ix.columns[col]; if (!(C.flags & 2)) continue;
-                int nu = 0;
-                for (int i = 0; i < nk; i++) { int id = C.value_id[sh.keep_doc[i]]; if (id < 0) continue; if (C.dict.off[id + 1] == C.dict.off[id]) continue;
-                    int u = 0; for (; u < nu; u++) if (sh.fv[u] == id) { sh.fc[u]++; break; } if (u == nu) { sh.fv[nu] = id; sh.fc[nu] = 1; nu++; } }
-                // OrderByDescending(count).ThenBy(key): stable insertion sort; key order = case-insensitive, then lower-case first (SURVEY Q12)
-                for (int a = 1; a < nu; a++) { int v = sh.fv[a], cn = sh.fc[a]; int b = a - 1;
-                    while (b >= 0) { bool gt;
-                        if (sh.fc[b] != cn) gt = sh.fc[b] < cn;
-                        else { Str x{C.dict.chars + C.dict.off[sh.fv[b]], (int)(C.dict.off[sh.fv[b] + 1] - C.dict.off[sh.fv[b]])}, y{C.dict.chars + C.dict.off[v], (int)(C.dict.off[v + 1] - C.dict.off[v])};
-                            int cv = cmp_ic_str(ix, x, y); if (cv == 0) cv = -cmp_ordinal(x.p, x.n, y.p, y.n); gt = cv > 0; }
-                        if (!gt) break; sh.fv[b + 1] = sh.fv[b]; sh.fc[b + 1] = sh.fc[b]; b--; }
-                    sh.fv[b + 1] = v; sh.fc[b + 1] = cn; }
-                int lim = nu < 100 ? nu : 100;
-                for (int u = 0; u < lim; u++) { if (nf < O.fcap) { size_t fo = (size_t)q * O.fcap + nf; O.facet_col[fo] = col; O.facet_val[fo] = sh.fv[u]; O.facet_cnt[fo] = sh.fc[u]; nf++; } else status |= 4; }
-            }
+        // shards: the hosts count the facets of the records they keep; a whole Stage-1 list is counted here in full (no cut at 100 values per
+        // column), for the hosts to sum over the shards -- at most fcap rows (more sets IFX_Q_OVERFLOW, as an unsharded table over fcap does)
+        if (p.enable_facets && O.fcap > 0 && nk > 0 && !(O.shard_info && (browse || host_filter))) {
+            const int32_t* kd = sh.keep_doc;
+            nf = facet_table(ix, nk, [&](int col, int i) { return ix.columns[col].value_id[kd[i]]; }, [](int) { return 1; }, O.shard_info ? 0x7fffffff : 100,
+                             sh.fv, sh.fc, O.facet_col + (size_t)q * O.fcap, O.facet_val + (size_t)q * O.fcap, O.facet_cnt + (size_t)q * O.fcap, O.fcap, status);
         }
         if (mode == 1 && p.short_kind != 0 && p.filter_id < 0 && B.s1_total && B.s1_total[q] > nk) nk = B.s1_total[q];      // the reference returns the WHOLE short-query list: TotalCandidates counts it
         O.n_facets[q] = nf; O.total[q] = browse ? 0 : nk;       // (TotalCandidates is not set on the browse path)
         int nout = nk < p.max_results ? nk : p.max_results; if (nout > O.cap) nout = O.cap; if (nout > n_rec && !browse && p.filter_id < 0) nout = n_rec;
         for (int i = 0; i < nout; i++) { size_t oo = (size_t)q * O.cap + i; O.key[oo] = ix.doc_key[sh.keep_doc[i]]; O.score[oo] = sh.keep_score[i]; O.tie[oo] = sh.keep_tie[i]; }
+        if (O.rec_post) {      // shards: per record the filter outcome (evaluated by the shard that owns the document) and its facet value ids
+            const bool flt = host_filter && p.filter_id >= 0 && p.filter_id < n_filters; bool unsupported = false;
+            for (int i = 0; i < nout; i++) { int32_t* r = O.rec_post + ((size_t)q * O.cap + i) * O.rec_stride; const int d = sh.keep_doc[i];
+                r[0] = flt ? (filter_exec(ix, filters[p.filter_id], d, unsupported) ? 1 : 0) : 1;
+                int k = 1;
+                for (int col = 0; col < ix.n_columns; col++) { const Column& C = ix.columns[col]; if (!(C.flags & 2)) continue;
+                    const int id = C.value_id[d]; r[k++] = (id >= 0 && C.dict.off[id + 1] != C.dict.off[id]) ? id : -1; } }
+            if (unsupported) status |= 2;
+        }
         O.n[q] = nout; O.status[q] = status;
     }
     c.sync();

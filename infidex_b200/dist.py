@@ -4,14 +4,18 @@ Layout (SURVEY.md 8e, DESIGN.md "multi-GPU"): rank r indexes the contiguous docu
 65 536 (the reference's container size, so no 4096-chunk of Bm25Scorer is ever split). The statistics the search path reads as global
 quantities -- term ordinals, df / idf, N, avgdl, word idf, prefix-set cardinalities, the affix dictionary -- are exchanged once at build
 time (ifx_builder_export_stats -> all_gather -> ifx_builder_globalize), and so are the champion lists of the one-character queries
-(ifx_builder_export_champions -> all_gather -> ifx_builder_globalize_champions). Every batch then runs on every shard, with these exchanges:
+(ifx_builder_export_champions -> all_gather -> ifx_builder_globalize_champions), and so are the filter / facet / sort column dictionaries
+(ifx_builder_export_columns -> all_gather -> ifx_builder_globalize_columns: a value id means the same on every shard). Every batch then
+runs on every shard, with these exchanges:
     all-reduce(sum)  document frequency of every LD1 union (its idf is a corpus-level quantity)                 16 int32 per query
     all-reduce(sum)  the selector's cardinalities                                                               40 int32 per query
     all-reduce(sum)  matched documents of every short query (only when the batch holds one)                     1 int32 per short query
     all-reduce(max)  largest integer score of every short query (BuildFinalScores)                              1 int32 per short query
     all-reduce(max)  largest coverage word hits per query (only with short queries: their fallback to Stage 1)   1 int32 per query
     all-gather       per-shard Stage-1 top-`depth` (key, score): global cut + global top score (normBm25)      depth * 12 B per query and shard
-    all-gather       per-shard final records (key, score, tie, counts, facet rows): merged identically on every rank
+    all-gather       per-shard final records (key, score, tie, counts): merged identically on every rank, truncated, then filtered
+    all-gather       per record: filter outcome + facet value ids (only when a query filters or counts facets)  4 * (1 + F) B per record
+    all-gather       facet rows of queries answered with their whole Stage-1 list (only those with facets)   12 * facet_cap B per query
 What is NOT exchanged (counted, never hidden -- `parity` in the bench line is the number of sampled queries whose merged records differ
 from the unsharded oracle): the selector's tier rules and the MaxScore threshold chain run on shard-local counts / heaps, the WordMatcher
 quota, docIndex-0/1 rule and truncation index are evaluated per shard.
@@ -100,6 +104,16 @@ class ShardedSearchEngine:
         rc = eng._host.ifx_builder_globalize_champions(C.c_void_p(eng._builder), self.world, self.rank, carr)
         if rc:
             raise E.NativeError("ifx_builder_globalize_champions failed (%d)" % rc)
+        # fourth exchange: the filter / facet / sort column dictionaries, so that a value id means the same on every shard
+        eng._host.ifx_builder_export_columns.restype = C.c_void_p
+        vp = eng._host.ifx_builder_export_columns(C.c_void_p(eng._builder), C.byref(n))
+        vblobs = self._all_gather_blob(np.ctypeslib.as_array((C.c_uint8 * n.value).from_address(vp)).copy())
+        varr = (C.c_void_p * self.world)(*[bl.ctypes.data for bl in vblobs])
+        rc = eng._host.ifx_builder_globalize_columns(C.c_void_p(eng._builder), self.world, self.rank, varr)
+        if rc:
+            raise E.NativeError("ifx_builder_globalize_columns failed (%d)" % rc)
+        colf = [f for f in schema if f.Filterable or f.Facetable or getattr(f, "Sortable", False)]      # the image's columns, schema order
+        self._fcols = [c for c, f in enumerate(colf) if f.Facetable]
         eng._upload(eng._host.ifx_builder_image(C.c_void_p(eng._builder)))
 
     def _all_gather_blob(self, mine):
@@ -118,6 +132,7 @@ class ShardedSearchEngine:
         """Marshal + upload a batch once (bench `value`: inputs resident in HBM before the timed region); run it with SearchBatch(uploaded=...)."""
         eng = self.eng; packed = eng.PackBatch(queries); h = C.c_void_p()
         eng._check(eng._gpu.ifx_batch_upload(eng._index, packed["arr"], len(queries), C.byref(h)), "ifx_batch_upload")
+        eng._check(eng._gpu.ifx_batch_set_facet_cap(h, packed["out"].facet_cap), "ifx_batch_set_facet_cap")
         if packed["post"] is not None:      # boosts / SortBy on shards: the device flags those queries IFX_Q_UNSUPPORTED_OP
             eng._check(eng._gpu.ifx_batch_set_post(h, packed["post"]), "ifx_batch_set_post")
         return {"packed": packed, "h": h, "queries": queries}
@@ -147,6 +162,7 @@ class ShardedSearchEngine:
             if h is None:
                 h = C.c_void_p(); eng._check(g.ifx_batch_upload(eng._index, packed["arr"], nq, C.byref(h)), "ifx_batch_upload")
             self._cached_h = h
+            eng._check(g.ifx_batch_set_facet_cap(h, packed["out"].facet_cap), "ifx_batch_set_facet_cap")
             if packed.get("post") is not None:      # (a refill clears it) boosts / SortBy on shards: flagged IFX_Q_UNSUPPORTED_OP by the device
                 eng._check(g.ifx_batch_set_post(h, packed["post"]), "ifx_batch_set_post")
         st = stats if stats is not None else E.Stats()
@@ -178,11 +194,13 @@ class ShardedSearchEngine:
             ks = [torch.empty_like(key) for _ in range(W)]; ss = [torch.empty_like(score) for _ in range(W)]; ns = [torch.empty_like(n) for _ in range(W)]
             dist.all_gather(ks, key); dist.all_gather(ss, score); dist.all_gather(ns, n)
             self.last_s1_counts = ns          # every shard's Stage-1 list lengths of the last batch ([W] tensors of [nq]; diagnostics, tests)
-            lim = None
-            if kind is not None:      # a short query's list is cut where the unsharded one is: at max_results when it is one character or is_short3
+            # the global list is cut where the unsharded one is: an n-gram query's at its CoverageDepth (the row length K may be longer when
+            # another query's max_results is), a short query's at max_results when it is one character or is_short3
+            lim = torch.tensor([q.CoverageDepth for q in queries], dtype=torch.int64, device=self.dev).clamp(max=K)
+            if kind is not None:
                 mx = torch.tensor([q.MaxNumberOfRecordsToReturn for q in queries], dtype=torch.int64, device=self.dev).clamp(max=K)
                 kd = torch.from_numpy(kind).to(self.dev)
-                lim = torch.where(((kd & 3) == 1) | ((kd & 4) != 0), mx, torch.full_like(mx, K))
+                lim = torch.where(kd == 0, lim, torch.where(((kd & 3) == 1) | ((kd & 4) != 0), mx, torch.full_like(mx, K)))
             keep, gmax, nglob = self._global_cut(ks, ss, ns, nq, K, lim)
             self._keep, self._gmax = keep, gmax          # borrowed by the library until the last phase has run
             eng._check(g.ifx_batch_stage1_restrict(h, C.c_void_p(keep.data_ptr()), C.c_void_p(gmax.data_ptr()), C.c_void_p(nglob.data_ptr())), "stage1 restrict"); sync()
@@ -210,13 +228,18 @@ class ShardedSearchEngine:
             tp = time.perf_counter(); eng._check(g.ifx_batch_download(h, C.byref(packed["out"])), "ifx_batch_download")
             info = np.zeros((nq, 8), np.int32); dkey = np.zeros((nq, 2), np.int64)
             eng._check(g.ifx_batch_shard_info(h, E._p(info), E._p(dkey)), "shard info")
-            packed["bufs"]["info"], packed["bufs"]["dkey"] = info, dkey; self._acc("download", tp)
+            packed["bufs"]["info"], packed["bufs"]["dkey"] = info, dkey
+            post = None
+            if any(q.Filter is not None or q.EnableFacets for q in queries):      # per record: filter outcome and facet value ids, gathered as they are
+                post = torch.empty((nq, cap, 1 + len(self._fcols)), dtype=torch.int32, device=self.dev)
+                eng._check(g.ifx_batch_shard_records(h, C.c_void_p(post.data_ptr()), post.shape[2]), "shard records")
+            self._acc("download", tp)
+            t0 = time.perf_counter()
+            merged = self._merge(queries, packed["bufs"], cap, post, h)
         except Exception:
             if uploaded is None:
                 g.ifx_batch_free(h); self._cached_h = None
             raise
-        t0 = time.perf_counter()
-        merged = self._merge(queries, packed["bufs"], cap, kind)
         self.exchange_ms["final"] += 1e3 * (time.perf_counter() - t0)
         return merged if raw else self._results(queries, merged)
 
@@ -247,8 +270,10 @@ class ShardedSearchEngine:
         """Membership of this rank's Stage-1 entries in the global top-K by (score desc, key asc), and the global top score per query.
         Every shard's list is already in that order, so an entry's global rank is its local rank plus, per other shard, the number of
         entries ahead of it -- W - 1 binary searches over packed (score bits, inverted key) words instead of a sort of all W * K entries.
-        `lim` ([nq], optional): a shorter global list for some queries (short queries cut at max_results)."""
+        `lim` ([nq]): the global list length of every query (its CoverageDepth; short queries may be cut at max_results); None: K for all."""
         torch = self.torch; W = self.world; dev = ss[0].device
+        if lim is None:
+            lim = torch.full((nq,), K, dtype=torch.int64, device=dev)
         N = torch.stack(ns, 1).clamp(min=0, max=K)                                             # [nq, W]
         slot = torch.arange(K, device=dev).view(1, K)
         big = torch.iinfo(torch.int64).max
@@ -267,15 +292,17 @@ class ShardedSearchEngine:
             if o != self.rank:
                 grank += torch.searchsorted(negc[o], mine, right=False)
         valid = slot < N[:, self.rank].view(nq, 1)
-        keep = torch.where(valid & (grank < (K if lim is None else lim.view(nq, 1))), torch.where(grank == 0, 2, torch.where(grank == 1, 3, 1)), 0).to(torch.uint8).contiguous().view(-1)      # 2 / 3: global rank 0 / 1 (docIndex 0 / 1)
+        keep = torch.where(valid & (grank < lim.view(nq, 1)), torch.where(grank == 0, 2, torch.where(grank == 1, 3, 1)), 0).to(torch.uint8).contiguous().view(-1)      # 2 / 3: global rank 0 / 1 (docIndex 0 / 1)
         first = torch.stack([torch.where(N[:, r] > 0, ss[r].view(nq, K)[:, 0], torch.zeros((), dtype=ss[r].dtype, device=dev)) for r in range(W)], 1)
         gmax = first.max(dim=1).values.clamp(min=0).contiguous()
-        nglob = N.sum(1).clamp(max=K).to(torch.int32).contiguous()
+        nglob = torch.minimum(N.sum(1), lim).to(torch.int32).contiguous()
         return keep, gmax, nglob
 
     def _global_cut_sort(self, ks, ss, ns, nq, K, lim=None):
         """General form (keys beyond 32 bits): two stable sorts over all W * K entries."""
         torch = self.torch; W = self.world
+        if lim is None:
+            lim = torch.full((nq,), K, dtype=torch.int64, device=ss[0].device)
         S = torch.stack([s.view(nq, K) for s in ss], 1).reshape(nq, W * K); Kk = torch.stack([k.view(nq, K) for k in ks], 1).reshape(nq, W * K)
         N = torch.stack(ns, 1).clamp(min=0)                                                    # [nq, W]
         slot = torch.arange(K, device=S.device).view(1, 1, K).expand(nq, W, K)
@@ -285,8 +312,7 @@ class ShardedSearchEngine:
         i2 = torch.argsort(S1, dim=1, descending=True, stable=True)
         order = torch.gather(i1, 1, i2)[:, :K]                                                 # flat positions of the global top-K
         top_valid = torch.gather(valid, 1, order)
-        if lim is not None:
-            top_valid = top_valid & (torch.arange(K, device=S.device).view(1, K) < lim.view(nq, 1))
+        top_valid = top_valid & (torch.arange(K, device=S.device).view(1, K) < lim.view(nq, 1))
         mark = torch.zeros(nq, W * K, dtype=torch.uint8, device=S.device)
         flag = top_valid.to(torch.uint8); flag[:, 0] *= 2                                     # 2: global rank 0, 3: global rank 1 (docIndex 0 / 1)
         if K > 1:
@@ -294,11 +320,14 @@ class ShardedSearchEngine:
         mark.scatter_(1, order, flag)
         keep = mark.view(nq, W, K)[:, self.rank, :].contiguous().view(-1)
         gmax = S.max(dim=1).values.clamp(min=0).contiguous()
-        nglob = valid.sum(1).clamp(max=K).to(torch.int32).contiguous()
+        nglob = torch.minimum(valid.sum(1), lim).to(torch.int32).contiguous()
         return keep, gmax, nglob
 
-    def _merge(self, queries, bufs, cap, kind=None):
-        """All-gather of every shard's records; merged by ScoreEntry order (Score desc, Tiebreaker desc, DocumentId asc) and cut to max."""
+    def _merge(self, queries, bufs, cap, post=None, h=None):
+        """All-gather of every shard's records; merged by ScoreEntry order (Score desc, Tiebreaker desc, DocumentId asc), truncated
+        (CalculateTruncationIndex), filtered, and the facet table built over what is left -- the order of SearchEngine.Search.
+        `post` ([nq, cap, 1 + facetable columns], device): per record of this shard its filter outcome and facet value ids, or None when no
+        query filters or counts facets. `h`: the batch handle (its device entry builds the facet tables)."""
         torch, dist, W = self.torch, self.dist, self.world
         import time
         nq = len(queries); eng = self.eng; tp = time.perf_counter()
@@ -307,19 +336,33 @@ class ShardedSearchEngine:
         meta = np.concatenate([np.stack([bufs["n"], bufs["total"], bufs["status"], bufs["nf"]], 1).astype(np.int64), bufs["info"].astype(np.int64), bufs["dkey"]], 1)      # [nq, 4 + 8 + 2]
         t_rec = torch.from_numpy(rec).to(self.dev); t_meta = torch.from_numpy(meta).to(self.dev)
         recs = [torch.empty_like(t_rec) for _ in range(W)]; metas = [torch.empty_like(t_meta) for _ in range(W)]
+        fq = np.array([q.EnableFacets for q in queries]); facets = bool(fq.any())
         self._acc("merge_pack", tp); tp = time.perf_counter()
         dist.all_gather(recs, t_rec); dist.all_gather(metas, t_meta)
+        if post is not None:
+            posts = [torch.empty_like(post) for _ in range(W)]; dist.all_gather(posts, post)
+        M = torch.stack(metas, 1)                                                                                                    # [nq, W, 14]
+        # a query answered with its WHOLE Stage-1 list (shard_info[6] == -1) was filtered on the shards: TotalCandidates and facet rows are summed
+        lst = (M[:, :, 10] == -1).cpu().numpy(); whole = lst.any(1)
+        sel = np.nonzero(whole & fq)[0]          # the same on every rank (from the gathered facts): each shard's facet rows of those queries
+        if len(sel):
+            fr = np.stack([bufs["fcol"][sel], bufs["fval"][sel], np.where(np.arange(bufs["fcnt"].shape[1])[None, :] < bufs["nf"][sel, None], bufs["fcnt"][sel], 0)], 2).astype(np.int32)
+            mine = torch.from_numpy(np.ascontiguousarray(fr)).to(self.dev); srows = [torch.empty_like(mine) for _ in range(W)]; dist.all_gather(srows, mine)
         if self.dev.type == "cuda":
             torch.cuda.synchronize(self.dev)
         self._acc("merge_gather", tp); tp = time.perf_counter()
         # merge on the device: ScoreEntry order (Score desc, Tiebreaker desc, DocumentId asc) = three stable sorts, least significant key first
-        R = torch.stack(recs, 1).reshape(nq, W * cap, 3); M = torch.stack(metas, 1)                                                   # [nq, W*cap, 3], [nq, W, 14]
+        R = torch.stack(recs, 1).reshape(nq, W * cap, 3)                                                                             # [nq, W*cap, 3]
         valid = (torch.arange(cap, device=self.dev).view(1, 1, cap) < M[:, :, 0:1]).reshape(nq, W * cap)
         key = R[:, :, 0].to(torch.int64); sbits = R[:, :, 1].to(torch.int64); tie = R[:, :, 2].to(torch.int64)
         score = torch.where(valid, sbits.to(torch.int32).view(torch.float32).to(torch.float64), torch.full((), float("-inf"), dtype=torch.float64, device=self.dev))
         o1 = torch.argsort(key, dim=1, stable=True)
         o2 = torch.gather(o1, 1, torch.argsort(torch.gather(-tie, 1, o1), dim=1, stable=True))
         order = torch.gather(o2, 1, torch.argsort(torch.gather(-score, 1, o2), dim=1, stable=True))[:, :cap]
+        # the blank query with EnableFacets (shard_info[6] == -2) browses the corpus in internal-id order: the shards' records in shard order
+        browse = (M[:, :, 10] == -2).any(1)
+        if bool(browse.any()):
+            order = torch.where(browse.view(nq, 1), torch.argsort((~valid).to(torch.int8), dim=1, stable=True)[:, :cap], order)
         t_key = torch.gather(key, 1, order); t_sbits = torch.gather(sbits, 1, order); t_tie = torch.gather(tie, 1, order); nvalid = valid.sum(1)
         maxr = torch.tensor([q.MaxNumberOfRecordsToReturn for q in queries], dtype=torch.int64, device=self.dev)
         # ResultProcessor.CalculateTruncationIndex over the merged list: the last record with Score >= 254 (records are sorted: the first n_ge),
@@ -338,36 +381,50 @@ class ShardedSearchEngine:
         status_t = M[:, 0, 2].clone()
         for r in range(1, W):
             status_t |= M[:, r, 2]
+        P = None
+        if post is not None:      # ApplyFilter after the truncation: the records that fail leave, TotalCandidates counts the rest (Take(max) is then a no-op)
+            S = post.shape[2]
+            P = torch.gather(torch.stack(posts, 1).reshape(nq, W * cap, S), 1, order.unsqueeze(2).expand(nq, cap, S))
+            kept = (P[:, :, 0] == 1) & (pos_idx < t_n.view(nq, 1))
+            ko = torch.argsort((~kept).to(torch.int8), dim=1, stable=True)
+            t_key = torch.gather(t_key, 1, ko); t_sbits = torch.gather(t_sbits, 1, ko); t_tie = torch.gather(t_tie, 1, ko); P = torch.gather(P, 1, ko.unsqueeze(2).expand(nq, cap, S))
+            t_n = kept.sum(1)
         o_key = t_key.cpu().numpy(); o_score = t_sbits.to(torch.int32).cpu().numpy().view(np.float32); o_tie = t_tie.to(torch.uint8).cpu().numpy(); o_n = t_n.cpu().numpy()
-        total = o_n.copy(); status = status_t.cpu().numpy(); self._acc("merge_sort_cut", tp)
+        total = np.where(browse.cpu().numpy(), 0, o_n)          # (TotalCandidates is not set on the browse path)
+        self._acc("merge_sort_cut", tp); tp = time.perf_counter()
         self.last_shard_info = M[:, :, 4:12]          # every shard's truncation facts of the last batch ([nq, W, 8]; diagnostics, tests)
-        if kind is not None:      # a short query whose records are its Stage-1 list (shard_info[6] == -1): TotalCandidates counts the whole list
-            lst = (M[:, :, 10] == -1).cpu().numpy(); short = kind != 0
-            total = np.where(short & lst.any(1), M[:, :, 1].sum(1).cpu().numpy(), total)
-            status = np.where(short & lst.any(1) & ~lst.all(1), status | 2, status)      # shards that disagree on the answer's kind: flagged, never mixed
+        total = np.where(whole, M[:, :, 1].sum(1).cpu().numpy(), total)      # TotalCandidates counts the whole list
+        facet_out = None
+        if facets:      # FacetBuilder over the records kept (one row per record and facetable column), or the summed rows of a whole Stage-1 list
+            nfc = len(self._fcols); fc = max(int(bufs["fcol"].shape[1]), 1)
+            cols = torch.tensor(self._fcols, dtype=torch.int32, device=self.dev).view(1, 1, nfc).expand(nq, cap, nfc)
+            ids = P[:, :, 1:]; cnt = ((pos_idx < t_n.view(nq, 1)).view(nq, cap, 1) & (ids >= 0)).to(torch.int32)
+            rows = torch.stack([cols, ids, cnt], 3).reshape(nq, cap * nfc, 3)
+            if len(sel):
+                sr = torch.stack(srows, 1).reshape(len(sel), W * mine.shape[1], 3); m = max(rows.shape[1], sr.shape[1])
+                rows = torch.nn.functional.pad(rows, (0, 0, 0, m - rows.shape[1])).clone()
+                rows[torch.from_numpy(sel).to(self.dev)] = torch.nn.functional.pad(sr, (0, 0, 0, m - sr.shape[1]))
+            rows = rows.contiguous(); m = rows.shape[1]
+            f_col = torch.zeros((nq, fc), dtype=torch.int32, device=self.dev); f_val = torch.zeros_like(f_col); f_cnt = torch.zeros_like(f_col)
+            f_n = torch.zeros(nq, dtype=torch.int32, device=self.dev); st32 = status_t.to(torch.int32).contiguous()
+            p_ = lambda t: C.c_void_p(t.data_ptr())
+            eng._check(eng._gpu.ifx_batch_facet_table(h, p_(rows), m, p_(f_col), p_(f_val), p_(f_cnt), p_(f_n), p_(st32)), "ifx_batch_facet_table")
+            status_t = st32.to(torch.int64)
+            facet_out = (f_col.cpu().numpy(), f_val.cpu().numpy(), f_cnt.cpu().numpy(), f_n.cpu().numpy())
+        status = status_t.cpu().numpy()
+        status = np.where(whole & ~lst.all(1), status | 2, status)      # shards that disagree on the answer's kind: flagged, never mixed
+        self._acc("merge_facets", tp)
         self.last_raw = (o_key, o_score, o_tie, o_n, total, status)
-        facets_all = None
-        if any(q.EnableFacets for q in queries):          # facet rows travel as strings (value ids are per-shard dictionaries)
-            mine = []
-            for i in range(nq):
-                rows = []
-                for k in range(int(bufs["nf"][i])):
-                    col = int(bufs["fcol"][i, k]); rows.append((eng._columns[col], eng._facet_value(col, int(bufs["fval"][i, k])), int(bufs["fcnt"][i, k])))
-                mine.append(rows)
-            facets_all = [None] * W
-            dist.all_gather_object(facets_all, mine)
-        return o_key, o_score, o_tie, o_n, total, status, facets_all
+        return o_key, o_score, o_tie, o_n, total, status, facet_out
 
     def _results(self, queries, merged):
-        o_key, o_score, o_tie, o_n, total, status, facets_all = merged; out = []
+        o_key, o_score, o_tie, o_n, total, status, facet_out = merged; out = []
         for i, q in enumerate(queries):
             records = [E.ScoreEntry(o_score[i, k], o_key[i, k], o_tie[i, k]) for k in range(int(o_n[i]))]
             facets = None
             if q.EnableFacets:
-                acc = {}
-                for r in range(self.world):
-                    for f, v, cnt in facets_all[r][i]:
-                        acc.setdefault(f, {}); acc[f][v] = acc[f].get(v, 0) + cnt
-                facets = {f: sorted(vs.items(), key=lambda kv: (-kv[1], kv[0].lower(), kv[0]))[:100] for f, vs in acc.items()}
+                f_col, f_val, f_cnt, f_n = facet_out; facets = {}
+                for k in range(int(f_n[i])):
+                    col = int(f_col[i, k]); facets.setdefault(self.eng._columns[col], []).append((self.eng._facet_value(col, int(f_val[i, k])), int(f_cnt[i, k])))
             out.append(E.Result(records, facets, int(total[i]), int(status[i])))
         return out
