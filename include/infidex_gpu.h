@@ -210,8 +210,10 @@ void ifx_batch_free(ifx_batch* b);
  * exchange data. phase 1: query preparation + LD1 expansion; then all-reduce(sum) of ifx_batch_fuzzy_df (document frequency of every LD1
  * union: its idf is a corpus-level quantity). phase 2: count pass of the candidate selection; all-reduce(sum) of ifx_batch_select_counts (the tier
  * rules compare corpus-level cardinalities). phase 3: selection, tf lookups, scoring; then all-gather of ifx_batch_stage1_lists and
- * ifx_batch_stage1_restrict (global top-`depth` cut, global top score for normBm25). phase 3: WordMatcher, coverage / fusion, truncation,
- * filter, facets; ifx_batch_download gives the shard's records, which every host merges after an all-gather.
+ * ifx_batch_stage1_restrict (global top-`depth` cut, global top score for normBm25). phase 4: WordMatcher lookups; ifx_batch_wm_counts
+ * and ifx_batch_wm_apply. phase 5: coverage / fusion, truncation, filter, facets; ifx_batch_download gives the shard's records, which every
+ * host merges after an all-gather. Phase 1, like ifx_batch_run, starts the run from the state of one GPU: nothing the exchange calls or
+ * phase 5 set for the previous batch carries over, so a handle run as a shard and then by ifx_batch_run answers as one GPU.
  * buf / key / score / n / keep / gmax are DEVICE pointers. */
 int  ifx_batch_run_phase(ifx_batch* b, int phase, ifx_stats* st);
 int  ifx_batch_fuzzy_df(ifx_batch* b, int32_t* buf /* [nq * 16] */, int set);

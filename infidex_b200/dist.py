@@ -20,8 +20,9 @@ What is NOT exchanged (counted, never hidden -- `parity` in the bench line is th
 from the unsharded oracle): the selector's tier rules and the MaxScore threshold chain run on shard-local counts / heaps, the WordMatcher
 quota, docIndex-0/1 rule and truncation index are evaluated per shard.
 """
+import contextlib
 import ctypes as C
-import os
+import time
 
 import numpy as np
 
@@ -51,6 +52,32 @@ def gather_results(dist, keys, device="cpu"):
     return [o.cpu().numpy() for o in out]
 
 
+def all_gather_blob(dist, mine, device="cpu"):
+    """Every rank's byte blob (sizes differ): the sizes, then one all-gather padded to the largest."""
+    import torch
+    world = dist.get_world_size()
+    sizes = [torch.zeros(1, dtype=torch.int64, device=device) for _ in range(world)]
+    dist.all_gather(sizes, torch.tensor([len(mine)], dtype=torch.int64, device=device))
+    sizes = [int(s.item()) for s in sizes]; cap = max(max(sizes), 1)
+    pad = np.zeros(cap, np.uint8); pad[: len(mine)] = mine
+    bufs = [torch.empty(cap, dtype=torch.uint8, device=device) for _ in range(world)]
+    dist.all_gather(bufs, torch.from_numpy(pad).to(device))
+    return [b.cpu().numpy()[: sizes[i]].copy() for i, b in enumerate(bufs)]
+
+
+def exchange_builder(dist, eng, export, globalize, device="cpu"):
+    """One build-time exchange between the shards' host builders: this shard's blob from the entry `export`, every shard's blob
+    (all_gather_blob), then the entry `globalize` over them, in rank order. Returns the blobs."""
+    n = C.c_size_t(0); ex = getattr(eng._host, export); ex.restype = C.c_void_p
+    p = ex(C.c_void_p(eng._builder), C.byref(n))
+    blobs = all_gather_blob(dist, np.ctypeslib.as_array((C.c_uint8 * n.value).from_address(p)).copy(), device)
+    arr = (C.c_void_p * len(blobs))(*[b.ctypes.data for b in blobs])
+    rc = getattr(eng._host, globalize)(C.c_void_p(eng._builder), len(blobs), dist.get_rank(), arr)
+    if rc:
+        raise E.NativeError("%s failed (%d)" % (globalize, rc))
+    return blobs
+
+
 def shard_ranges(n_docs, world):
     """Contiguous doc-id ranges on 65 536-document boundaries (every shard non-empty when n_docs >= world * 65 536)."""
     nc = (n_docs + CONTAINER - 1) // CONTAINER
@@ -73,69 +100,36 @@ class ShardedSearchEngine:
     # ---- build -------------------------------------------------------------------------------------------------------------------------
     def IndexShard(self, keys, schema, columns, threads=None):
         """`keys` / `columns`: this rank's document range only (ranks in doc order)."""
-        eng, torch, dist = self.eng, self.torch, self.dist
+        eng, dist = self.eng, self.dist
         eng.IndexColumns(keys, schema, columns, threads=threads, upload=False)
-        n = C.c_size_t(0)
-        eng._host.ifx_builder_export_stats.restype = C.c_void_p
-        p = eng._host.ifx_builder_export_stats(C.c_void_p(eng._builder), C.byref(n))
-        mine = np.ctypeslib.as_array((C.c_uint8 * n.value).from_address(p)).copy()
-        blobs = self._all_gather_blob(mine)
-        arr = (C.c_void_p * self.world)(*[bl.ctypes.data for bl in blobs])
-        rc = eng._host.ifx_builder_globalize(C.c_void_p(eng._builder), self.world, self.rank, arr)
-        if rc:
-            raise E.NativeError("ifx_builder_globalize failed (%d)" % rc)
-        # second exchange: document lengths after the corpus-level stop terms were dropped -> avgdl (one sequential float sum, as the reference)
+        exchange_builder(dist, eng, "ifx_builder_export_stats", "ifx_builder_globalize", self.dev)
+        # document lengths after the corpus-level stop terms were dropped -> avgdl (one sequential float sum, as the reference)
         cnt = C.c_int(0); eng._host.ifx_builder_doc_lengths.restype = C.c_void_p
         lp = eng._host.ifx_builder_doc_lengths(C.c_void_p(eng._builder), C.byref(cnt))
-        mine_l = np.ctypeslib.as_array((C.c_float * max(cnt.value, 1)).from_address(lp))[: cnt.value].copy()
-        nsz = [torch.zeros(1, dtype=torch.int64, device=self.dev) for _ in range(self.world)]
-        dist.all_gather(nsz, torch.tensor([cnt.value], dtype=torch.int64, device=self.dev)); nsz = [int(x.item()) for x in nsz]; capl = max(max(nsz), 1)
-        padl = np.zeros(capl, np.float32); padl[: cnt.value] = mine_l
-        lb = [torch.empty(capl, dtype=torch.float32, device=self.dev) for _ in range(self.world)]
-        dist.all_gather(lb, torch.from_numpy(padl).to(self.dev))
-        lens = [np.ascontiguousarray(x.cpu().numpy()[: nsz[i]]) for i, x in enumerate(lb)]
-        larr = (C.c_void_p * self.world)(*[x.ctypes.data for x in lens]); carr = (C.c_int * self.world)(*nsz)
+        mine = np.ctypeslib.as_array((C.c_float * max(cnt.value, 1)).from_address(lp))[: cnt.value].copy()
+        lens = [b.view(np.float32) for b in all_gather_blob(dist, mine.view(np.uint8), self.dev)]
+        larr = (C.c_void_p * self.world)(*[x.ctypes.data for x in lens]); carr = (C.c_int * self.world)(*[len(x) for x in lens])
         eng._host.ifx_builder_set_global_lengths(C.c_void_p(eng._builder), self.world, larr, carr)
-        # third exchange: the champion lists of the one-character queries (every shard's candidates per first character -> the global lists)
-        eng._host.ifx_builder_export_champions.restype = C.c_void_p
-        cp = eng._host.ifx_builder_export_champions(C.c_void_p(eng._builder), C.byref(n))
-        cblobs = self._all_gather_blob(np.ctypeslib.as_array((C.c_uint8 * n.value).from_address(cp)).copy())
-        carr = (C.c_void_p * self.world)(*[bl.ctypes.data for bl in cblobs])
-        rc = eng._host.ifx_builder_globalize_champions(C.c_void_p(eng._builder), self.world, self.rank, carr)
-        if rc:
-            raise E.NativeError("ifx_builder_globalize_champions failed (%d)" % rc)
-        # fourth exchange: the filter / facet / sort column dictionaries, so that a value id means the same on every shard
-        eng._host.ifx_builder_export_columns.restype = C.c_void_p
-        vp = eng._host.ifx_builder_export_columns(C.c_void_p(eng._builder), C.byref(n))
-        vblobs = self._all_gather_blob(np.ctypeslib.as_array((C.c_uint8 * n.value).from_address(vp)).copy())
-        varr = (C.c_void_p * self.world)(*[bl.ctypes.data for bl in vblobs])
-        rc = eng._host.ifx_builder_globalize_columns(C.c_void_p(eng._builder), self.world, self.rank, varr)
-        if rc:
-            raise E.NativeError("ifx_builder_globalize_columns failed (%d)" % rc)
+        exchange_builder(dist, eng, "ifx_builder_export_champions", "ifx_builder_globalize_champions", self.dev)      # the one-character queries' champion lists
+        exchange_builder(dist, eng, "ifx_builder_export_columns", "ifx_builder_globalize_columns", self.dev)          # a value id means the same on every shard
         colf = [f for f in schema if f.Filterable or f.Facetable or getattr(f, "Sortable", False)]      # the image's columns, schema order
         self._fcols = [c for c, f in enumerate(colf) if f.Facetable]
         eng._upload(eng._host.ifx_builder_image(C.c_void_p(eng._builder)))
-
-    def _all_gather_blob(self, mine):
-        """Every rank's byte blob (sizes differ): the sizes, then one all-gather padded to the largest."""
-        torch, dist = self.torch, self.dist
-        sizes = [torch.zeros(1, dtype=torch.int64, device=self.dev) for _ in range(self.world)]
-        dist.all_gather(sizes, torch.tensor([len(mine)], dtype=torch.int64, device=self.dev))
-        sizes = [int(s.item()) for s in sizes]; cap = max(sizes)
-        pad = np.zeros(cap, np.uint8); pad[: len(mine)] = mine
-        bufs = [torch.empty(cap, dtype=torch.uint8, device=self.dev) for _ in range(self.world)]
-        dist.all_gather(bufs, torch.from_numpy(pad).to(self.dev))
-        return [b.cpu().numpy()[: sizes[i]].copy() for i, b in enumerate(bufs)]
 
     # ---- search ------------------------------------------------------------------------------------------------------------------------
     def UploadBatch(self, queries):
         """Marshal + upload a batch once (bench `value`: inputs resident in HBM before the timed region); run it with SearchBatch(uploaded=...)."""
         eng = self.eng; packed = eng.PackBatch(queries); h = C.c_void_p()
         eng._check(eng._gpu.ifx_batch_upload(eng._index, packed["arr"], len(queries), C.byref(h)), "ifx_batch_upload")
-        eng._check(eng._gpu.ifx_batch_set_facet_cap(h, packed["out"].facet_cap), "ifx_batch_set_facet_cap")
-        if packed["post"] is not None:      # boosts / SortBy on shards: the device flags those queries IFX_Q_UNSUPPORTED_OP
-            eng._check(eng._gpu.ifx_batch_set_post(h, packed["post"]), "ifx_batch_set_post")
+        self._setup_handle(h, packed)
         return {"packed": packed, "h": h, "queries": queries}
+
+    def _setup_handle(self, h, packed):
+        """The batch's facet capacity, and its boosts / SortBy (a refill clears them), which the device flags IFX_Q_UNSUPPORTED_OP on shards."""
+        eng = self.eng
+        eng._check(eng._gpu.ifx_batch_set_facet_cap(h, packed["out"].facet_cap), "ifx_batch_set_facet_cap")
+        if packed["post"] is not None:
+            eng._check(eng._gpu.ifx_batch_set_post(h, packed["post"]), "ifx_batch_set_post")
 
     def FreeBatch(self, up):
         self.eng._gpu.ifx_batch_free(up["h"])
@@ -148,7 +142,6 @@ class ShardedSearchEngine:
 
     def SearchBatch(self, queries, stats=None, raw=False, uploaded=None, packed=None):
         """Every rank passes the SAME queries; every rank returns the same merged Results (Records, TotalCandidates, Facets by string)."""
-        import time
         eng, torch, dist, g = self.eng, self.torch, self.dist, self.eng._gpu
         if uploaded is not None:
             queries = uploaded["queries"]
@@ -162,109 +155,107 @@ class ShardedSearchEngine:
             if h is None:
                 h = C.c_void_p(); eng._check(g.ifx_batch_upload(eng._index, packed["arr"], nq, C.byref(h)), "ifx_batch_upload")
             self._cached_h = h
-            eng._check(g.ifx_batch_set_facet_cap(h, packed["out"].facet_cap), "ifx_batch_set_facet_cap")
-            if packed.get("post") is not None:      # (a refill clears it) boosts / SortBy on shards: flagged IFX_Q_UNSUPPORTED_OP by the device
-                eng._check(g.ifx_batch_set_post(h, packed["post"]), "ifx_batch_set_post")
+            self._setup_handle(h, packed)
         st = stats if stats is not None else E.Stats()
 
-        def sync():
-            if self.dev.type == "cuda":
-                torch.cuda.synchronize(self.dev)
+        def phase(k):
+            with self._timed(self.host_ms, "phase%d" % k):
+                eng._check(g.ifx_batch_run_phase(h, k, C.byref(st)), "phase %d" % k)
         try:
-            tp = time.perf_counter(); eng._check(g.ifx_batch_run_phase(h, 1, C.byref(st)), "phase 1"); self._acc("phase1", tp)
-            t0 = time.perf_counter()
-            fdf = torch.zeros(nq * 16, dtype=torch.int32, device=self.dev)
-            eng._check(g.ifx_batch_fuzzy_df(h, C.c_void_p(fdf.data_ptr()), 0), "fuzzy df get")
-            dist.all_reduce(fdf)
-            eng._check(g.ifx_batch_fuzzy_df(h, C.c_void_p(fdf.data_ptr()), 1), "fuzzy df set"); sync()
-            self.exchange_ms["fuzzy_df"] += 1e3 * (time.perf_counter() - t0)
-            tp = time.perf_counter(); eng._check(g.ifx_batch_run_phase(h, 2, C.byref(st)), "phase 2"); self._acc("phase2", tp)
-            t0 = time.perf_counter()
-            sc = torch.zeros(nq * 40, dtype=torch.int32, device=self.dev)
-            eng._check(g.ifx_batch_select_counts(h, C.c_void_p(sc.data_ptr()), 0), "select counts get")
-            dist.all_reduce(sc)
-            eng._check(g.ifx_batch_select_counts(h, C.c_void_p(sc.data_ptr()), 1), "select counts set"); sync()
-            self.exchange_ms["select_counts"] = self.exchange_ms.get("select_counts", 0.0) + 1e3 * (time.perf_counter() - t0)
-            tp = time.perf_counter(); eng._check(g.ifx_batch_run_phase(h, 3, C.byref(st)), "phase 3"); self._acc("phase3", tp)
+            phase(1)
+            self._round(h, "fuzzy_df", g.ifx_batch_fuzzy_df, nq * 16)
+            phase(2)
+            self._round(h, "select_counts", g.ifx_batch_select_counts, nq * 40)
+            phase(3)
             kind = self._short_queries(h, nq)
-            t0 = time.perf_counter()
-            key = torch.zeros(nq * K, dtype=torch.int64, device=self.dev); score = torch.zeros(nq * K, dtype=torch.float32, device=self.dev); n = torch.zeros(nq, dtype=torch.int32, device=self.dev)
-            eng._check(g.ifx_batch_stage1_lists(h, C.c_void_p(key.data_ptr()), C.c_void_p(score.data_ptr()), C.c_void_p(n.data_ptr())), "stage1 lists")
-            W = self.world
-            ks = [torch.empty_like(key) for _ in range(W)]; ss = [torch.empty_like(score) for _ in range(W)]; ns = [torch.empty_like(n) for _ in range(W)]
-            dist.all_gather(ks, key); dist.all_gather(ss, score); dist.all_gather(ns, n)
-            self.last_s1_counts = ns          # every shard's Stage-1 list lengths of the last batch ([W] tensors of [nq]; diagnostics, tests)
-            # the global list is cut where the unsharded one is: an n-gram query's at its CoverageDepth (the row length K may be longer when
-            # another query's max_results is), a short query's at max_results when it is one character or is_short3
-            lim = torch.tensor([q.CoverageDepth for q in queries], dtype=torch.int64, device=self.dev).clamp(max=K)
-            if kind is not None:
-                mx = torch.tensor([q.MaxNumberOfRecordsToReturn for q in queries], dtype=torch.int64, device=self.dev).clamp(max=K)
-                kd = torch.from_numpy(kind).to(self.dev)
-                lim = torch.where(kd == 0, lim, torch.where(((kd & 3) == 1) | ((kd & 4) != 0), mx, torch.full_like(mx, K)))
-            keep, gmax, nglob = self._global_cut(ks, ss, ns, nq, K, lim)
-            self._keep, self._gmax = keep, gmax          # borrowed by the library until the last phase has run
-            eng._check(g.ifx_batch_stage1_restrict(h, C.c_void_p(keep.data_ptr()), C.c_void_p(gmax.data_ptr()), C.c_void_p(nglob.data_ptr())), "stage1 restrict"); sync()
-            self.exchange_ms["stage1"] += 1e3 * (time.perf_counter() - t0)
-            tp = time.perf_counter(); eng._check(g.ifx_batch_run_phase(h, 4, C.byref(st)), "phase 4"); self._acc("phase4", tp)
-            t0 = time.perf_counter()
-            wc = torch.zeros(nq * 4, dtype=torch.int32, device=self.dev)
-            eng._check(g.ifx_batch_wm_counts(h, C.c_void_p(wc.data_ptr())), "wm counts")
-            wcs = [torch.empty_like(wc) for _ in range(W)]; dist.all_gather(wcs, wc)
-            WC = torch.stack([x.view(nq, 4) for x in wcs], 1)                                # [nq, W, 4]
-            depth = torch.tensor([q.CoverageDepth for q in queries], dtype=torch.int32, device=self.dev)
-            limit = (depth - WC[:, :, 0].sum(1)).clamp(min=0)                                 # wmLimit = coverageDepth - overlap over all shards
-            before = torch.cumsum(WC[:, :, 1], 1) - WC[:, :, 1]                               # WordMatcher-only documents of the lower shards come first (ascending ids)
-            allowed = (limit.view(nq, 1) - before).clamp(min=0)[:, self.rank].to(torch.int32).contiguous()
-            anyg = (WC[:, :, 2].sum(1) > 0).to(torch.int32).contiguous()
-            eng._check(g.ifx_batch_wm_apply(h, C.c_void_p(allowed.data_ptr()), C.c_void_p(anyg.data_ptr())), "wm apply"); sync()
-            self.exchange_ms["wm"] = self.exchange_ms.get("wm", 0.0) + 1e3 * (time.perf_counter() - t0)
+            with self._timed(self.exchange_ms, "stage1"):
+                key = torch.zeros(nq * K, dtype=torch.int64, device=self.dev); score = torch.zeros(nq * K, dtype=torch.float32, device=self.dev); n = torch.zeros(nq, dtype=torch.int32, device=self.dev)
+                eng._check(g.ifx_batch_stage1_lists(h, C.c_void_p(key.data_ptr()), C.c_void_p(score.data_ptr()), C.c_void_p(n.data_ptr())), "stage1 lists")
+                W = self.world
+                ks = [torch.empty_like(key) for _ in range(W)]; ss = [torch.empty_like(score) for _ in range(W)]; ns = [torch.empty_like(n) for _ in range(W)]
+                dist.all_gather(ks, key); dist.all_gather(ss, score); dist.all_gather(ns, n)
+                self.last_s1_counts = ns          # every shard's Stage-1 list lengths of the last batch ([W] tensors of [nq]; diagnostics, tests)
+                # the global list is cut where the unsharded one is: an n-gram query's at its CoverageDepth (the row length K may be longer when
+                # another query's max_results is), a short query's at max_results when it is one character or is_short3
+                lim = torch.tensor([q.CoverageDepth for q in queries], dtype=torch.int64, device=self.dev).clamp(max=K)
+                if kind is not None:
+                    mx = torch.tensor([q.MaxNumberOfRecordsToReturn for q in queries], dtype=torch.int64, device=self.dev).clamp(max=K)
+                    kd = torch.from_numpy(kind).to(self.dev)
+                    lim = torch.where(kd == 0, lim, torch.where(((kd & 3) == 1) | ((kd & 4) != 0), mx, torch.full_like(mx, K)))
+                keep, gmax, nglob = self._global_cut(ks, ss, ns, nq, K, lim)
+                self._keep, self._gmax = keep, gmax          # borrowed by the library until the last phase has run
+                eng._check(g.ifx_batch_stage1_restrict(h, C.c_void_p(keep.data_ptr()), C.c_void_p(gmax.data_ptr()), C.c_void_p(nglob.data_ptr())), "stage1 restrict"); self._sync()
+            phase(4)
+            with self._timed(self.exchange_ms, "wm"):
+                wc = torch.zeros(nq * 4, dtype=torch.int32, device=self.dev)
+                eng._check(g.ifx_batch_wm_counts(h, C.c_void_p(wc.data_ptr())), "wm counts")
+                wcs = [torch.empty_like(wc) for _ in range(W)]; dist.all_gather(wcs, wc)
+                WC = torch.stack([x.view(nq, 4) for x in wcs], 1)                                # [nq, W, 4]
+                depth = torch.tensor([q.CoverageDepth for q in queries], dtype=torch.int32, device=self.dev)
+                limit = (depth - WC[:, :, 0].sum(1)).clamp(min=0)                                 # wmLimit = coverageDepth - overlap over all shards
+                before = torch.cumsum(WC[:, :, 1], 1) - WC[:, :, 1]                               # WordMatcher-only documents of the lower shards come first (ascending ids)
+                allowed = (limit.view(nq, 1) - before).clamp(min=0)[:, self.rank].to(torch.int32).contiguous()
+                anyg = (WC[:, :, 2].sum(1) > 0).to(torch.int32).contiguous()
+                eng._check(g.ifx_batch_wm_apply(h, C.c_void_p(allowed.data_ptr()), C.c_void_p(anyg.data_ptr())), "wm apply"); self._sync()
             if kind is not None:      # short queries: coverage word hits over all shards decide the fallback to the Stage-1 list on every shard alike
-                t0 = time.perf_counter(); hits = torch.zeros(nq, dtype=torch.int32, device=self.dev)
-                eng._check(g.ifx_batch_short_hits(h, C.c_void_p(hits.data_ptr()), 0), "short hits get")
-                dist.all_reduce(hits, op=dist.ReduceOp.MAX)
-                eng._check(g.ifx_batch_short_hits(h, C.c_void_p(hits.data_ptr()), 1), "short hits set"); sync()
-                self.exchange_ms["short"] = self.exchange_ms.get("short", 0.0) + 1e3 * (time.perf_counter() - t0)
-            tp = time.perf_counter(); eng._check(g.ifx_batch_run_phase(h, 5, C.byref(st)), "phase 5"); self._acc("phase5", tp)
-            tp = time.perf_counter(); eng._check(g.ifx_batch_download(h, C.byref(packed["out"])), "ifx_batch_download")
-            info = np.zeros((nq, 8), np.int32); dkey = np.zeros((nq, 2), np.int64)
-            eng._check(g.ifx_batch_shard_info(h, E._p(info), E._p(dkey)), "shard info")
-            packed["bufs"]["info"], packed["bufs"]["dkey"] = info, dkey
-            post = None
-            if any(q.Filter is not None or q.EnableFacets for q in queries):      # per record: filter outcome and facet value ids, gathered as they are
-                post = torch.empty((nq, cap, 1 + len(self._fcols)), dtype=torch.int32, device=self.dev)
-                eng._check(g.ifx_batch_shard_records(h, C.c_void_p(post.data_ptr()), post.shape[2]), "shard records")
-            self._acc("download", tp)
-            t0 = time.perf_counter()
-            merged = self._merge(queries, packed["bufs"], cap, post, h)
+                self._round(h, "short", g.ifx_batch_short_hits, nq, dist.ReduceOp.MAX)
+            phase(5)
+            with self._timed(self.host_ms, "download"):
+                eng._check(g.ifx_batch_download(h, C.byref(packed["out"])), "ifx_batch_download")
+                info = np.zeros((nq, 8), np.int32); dkey = np.zeros((nq, 2), np.int64)
+                eng._check(g.ifx_batch_shard_info(h, E._p(info), E._p(dkey)), "shard info")
+                packed["bufs"]["info"], packed["bufs"]["dkey"] = info, dkey
+                post = None
+                if any(q.Filter is not None or q.EnableFacets for q in queries):      # per record: filter outcome and facet value ids, gathered as they are
+                    post = torch.empty((nq, cap, 1 + len(self._fcols)), dtype=torch.int32, device=self.dev)
+                    eng._check(g.ifx_batch_shard_records(h, C.c_void_p(post.data_ptr()), post.shape[2]), "shard records")
+            with self._timed(self.exchange_ms, "final"):
+                merged = self._merge(queries, packed["bufs"], cap, post, h)
         except Exception:
             if uploaded is None:
                 g.ifx_batch_free(h); self._cached_h = None
             raise
-        self.exchange_ms["final"] += 1e3 * (time.perf_counter() - t0)
         return merged if raw else self._results(queries, merged)
+
+    def _results(self, queries, merged):
+        """The Results (facets by string) of SearchBatch(raw=True)'s merged buffers."""
+        return self.eng._results(queries, *merged)
+
+    def _sync(self):
+        if self.dev.type == "cuda":
+            self.torch.cuda.synchronize(self.dev)
+
+    @contextlib.contextmanager
+    def _timed(self, acc, name):
+        """Adds the wall time of the block to acc[name] (ms)."""
+        t0 = time.perf_counter()
+        yield
+        acc[name] = acc.get(name, 0.0) + 1e3 * (time.perf_counter() - t0)
+
+    def _round(self, h, name, entry, n, op=None):
+        """One per-batch round: `entry` gets n int32 per shard into a device tensor, the hosts all-reduce it (sum unless `op`), `entry` sets it."""
+        with self._timed(self.exchange_ms, name):
+            buf = self.torch.zeros(n, dtype=self.torch.int32, device=self.dev); ptr = C.c_void_p(buf.data_ptr())
+            self.eng._check(entry(h, ptr, 0), "%s get" % name)
+            self.dist.all_reduce(buf, op=self.dist.ReduceOp.SUM if op is None else op)
+            self.eng._check(entry(h, ptr, 1), "%s set" % name); self._sync()
 
     def _short_queries(self, h, nq):
         """The short queries of the batch (no word of >= 3 characters), group by group: matched documents summed over the shards (fuzzy
         fallback below 100), then the largest integer score (BuildFinalScores). Returns the per-query kinds, or None when there is none --
         the device counts them from the texts, so every rank takes the same branch."""
-        import time
         eng, torch, dist, g = self.eng, self.torch, self.dist, self.eng._gpu
         ng = C.c_int(0); gs = C.c_int(0); kind = np.zeros(nq, np.int32)
         eng._check(g.ifx_batch_short_groups(h, E._p(kind), C.byref(ng), C.byref(gs)), "short groups")
         if ng.value == 0:
             return None
-        t0 = time.perf_counter()
-        buf = torch.zeros(gs.value, dtype=torch.int32, device=self.dev); ptr = C.c_void_p(buf.data_ptr())
-        for grp in range(ng.value):
-            eng._check(g.ifx_batch_short_step(h, 0, grp, ptr), "short step 0"); dist.all_reduce(buf)
-            eng._check(g.ifx_batch_short_step(h, 1, grp, ptr), "short step 1"); dist.all_reduce(buf, op=dist.ReduceOp.MAX)
-            eng._check(g.ifx_batch_short_step(h, 2, grp, ptr), "short step 2")
-        self.exchange_ms["short"] = self.exchange_ms.get("short", 0.0) + 1e3 * (time.perf_counter() - t0)
+        with self._timed(self.exchange_ms, "short"):
+            buf = torch.zeros(gs.value, dtype=torch.int32, device=self.dev); ptr = C.c_void_p(buf.data_ptr())
+            for grp in range(ng.value):
+                eng._check(g.ifx_batch_short_step(h, 0, grp, ptr), "short step 0"); dist.all_reduce(buf)
+                eng._check(g.ifx_batch_short_step(h, 1, grp, ptr), "short step 1"); dist.all_reduce(buf, op=dist.ReduceOp.MAX)
+                eng._check(g.ifx_batch_short_step(h, 2, grp, ptr), "short step 2")
         return kind
-
-    def _acc(self, name, t0):
-        import time
-        self.host_ms[name] = self.host_ms.get(name, 0.0) + 1e3 * (time.perf_counter() - t0)
 
     def _global_cut(self, ks, ss, ns, nq, K, lim=None):
         """Membership of this rank's Stage-1 entries in the global top-K by (score desc, key asc), and the global top score per query.
@@ -329,102 +320,89 @@ class ShardedSearchEngine:
         `post` ([nq, cap, 1 + facetable columns], device): per record of this shard its filter outcome and facet value ids, or None when no
         query filters or counts facets. `h`: the batch handle (its device entry builds the facet tables)."""
         torch, dist, W = self.torch, self.dist, self.world
-        import time
-        nq = len(queries); eng = self.eng; tp = time.perf_counter()
-        rec = np.zeros((nq, cap, 3), np.float64)          # key, score bits (exact in f64), tie
-        rec[:, :, 0] = bufs["keys"]; rec[:, :, 1] = bufs["scores"].view(np.uint32).astype(np.float64); rec[:, :, 2] = bufs["ties"]
-        meta = np.concatenate([np.stack([bufs["n"], bufs["total"], bufs["status"], bufs["nf"]], 1).astype(np.int64), bufs["info"].astype(np.int64), bufs["dkey"]], 1)      # [nq, 4 + 8 + 2]
-        t_rec = torch.from_numpy(rec).to(self.dev); t_meta = torch.from_numpy(meta).to(self.dev)
-        recs = [torch.empty_like(t_rec) for _ in range(W)]; metas = [torch.empty_like(t_meta) for _ in range(W)]
-        fq = np.array([q.EnableFacets for q in queries]); facets = bool(fq.any())
-        self._acc("merge_pack", tp); tp = time.perf_counter()
-        dist.all_gather(recs, t_rec); dist.all_gather(metas, t_meta)
-        if post is not None:
-            posts = [torch.empty_like(post) for _ in range(W)]; dist.all_gather(posts, post)
-        M = torch.stack(metas, 1)                                                                                                    # [nq, W, 14]
-        # a query answered with its WHOLE Stage-1 list (shard_info[6] == -1) was filtered on the shards: TotalCandidates and facet rows are summed
-        lst = (M[:, :, 10] == -1).cpu().numpy(); whole = lst.any(1)
-        sel = np.nonzero(whole & fq)[0]          # the same on every rank (from the gathered facts): each shard's facet rows of those queries
-        if len(sel):
-            fr = np.stack([bufs["fcol"][sel], bufs["fval"][sel], np.where(np.arange(bufs["fcnt"].shape[1])[None, :] < bufs["nf"][sel, None], bufs["fcnt"][sel], 0)], 2).astype(np.int32)
-            mine = torch.from_numpy(np.ascontiguousarray(fr)).to(self.dev); srows = [torch.empty_like(mine) for _ in range(W)]; dist.all_gather(srows, mine)
-        if self.dev.type == "cuda":
-            torch.cuda.synchronize(self.dev)
-        self._acc("merge_gather", tp); tp = time.perf_counter()
-        # merge on the device: ScoreEntry order (Score desc, Tiebreaker desc, DocumentId asc) = three stable sorts, least significant key first
-        R = torch.stack(recs, 1).reshape(nq, W * cap, 3)                                                                             # [nq, W*cap, 3]
-        valid = (torch.arange(cap, device=self.dev).view(1, 1, cap) < M[:, :, 0:1]).reshape(nq, W * cap)
-        key = R[:, :, 0].to(torch.int64); sbits = R[:, :, 1].to(torch.int64); tie = R[:, :, 2].to(torch.int64)
-        score = torch.where(valid, sbits.to(torch.int32).view(torch.float32).to(torch.float64), torch.full((), float("-inf"), dtype=torch.float64, device=self.dev))
-        o1 = torch.argsort(key, dim=1, stable=True)
-        o2 = torch.gather(o1, 1, torch.argsort(torch.gather(-tie, 1, o1), dim=1, stable=True))
-        order = torch.gather(o2, 1, torch.argsort(torch.gather(-score, 1, o2), dim=1, stable=True))[:, :cap]
-        # the blank query with EnableFacets (shard_info[6] == -2) browses the corpus in internal-id order: the shards' records in shard order
-        browse = (M[:, :, 10] == -2).any(1)
-        if bool(browse.any()):
-            order = torch.where(browse.view(nq, 1), torch.argsort((~valid).to(torch.int8), dim=1, stable=True)[:, :cap], order)
-        t_key = torch.gather(key, 1, order); t_sbits = torch.gather(sbits, 1, order); t_tie = torch.gather(tie, 1, order); nvalid = valid.sum(1)
-        maxr = torch.tensor([q.MaxNumberOfRecordsToReturn for q in queries], dtype=torch.int64, device=self.dev)
-        # ResultProcessor.CalculateTruncationIndex over the merged list: the last record with Score >= 254 (records are sorted: the first n_ge),
-        # or a docIndex-0/1 document whose word hits reach max(1, max word hits over all shards) or whose lcs is non-zero
-        info = M[:, :, 4:12]; dk = M[:, :, 12:14]
-        min_hits = info[:, :, 0].max(1).values.clamp(min=1); trunc = info[:, :, 1].sum(1) - 1
-        pos_idx = torch.arange(cap, device=self.dev).view(1, cap)
-        for j in range(2):
-            wh = info[:, :, 2 + 2 * j].max(1).values; lc = info[:, :, 3 + 2 * j].max(1).values; dkj = dk[:, :, j].max(1).values      # the owner reports >= 0, the others -1
-            qual = (wh >= 0) & ((wh >= min_hits) | (lc > 0))
-            hit = (t_key == dkj.view(nq, 1)) & (pos_idx < nvalid.clamp(max=cap).view(nq, 1))
-            pos = torch.where(hit.any(1), hit.to(torch.int64).argmax(1), torch.full((), cap, dtype=torch.int64, device=self.dev))      # beyond the merged top: at least `cap`
-            trunc = torch.where(qual, torch.maximum(trunc, pos), trunc)
-        count = torch.where(trunc < 0, maxr, torch.minimum(trunc + 1, maxr))
-        t_n = torch.minimum(torch.minimum(nvalid, count), maxr)
-        status_t = M[:, 0, 2].clone()
-        for r in range(1, W):
-            status_t |= M[:, r, 2]
-        P = None
-        if post is not None:      # ApplyFilter after the truncation: the records that fail leave, TotalCandidates counts the rest (Take(max) is then a no-op)
-            S = post.shape[2]
-            P = torch.gather(torch.stack(posts, 1).reshape(nq, W * cap, S), 1, order.unsqueeze(2).expand(nq, cap, S))
-            kept = (P[:, :, 0] == 1) & (pos_idx < t_n.view(nq, 1))
-            ko = torch.argsort((~kept).to(torch.int8), dim=1, stable=True)
-            t_key = torch.gather(t_key, 1, ko); t_sbits = torch.gather(t_sbits, 1, ko); t_tie = torch.gather(t_tie, 1, ko); P = torch.gather(P, 1, ko.unsqueeze(2).expand(nq, cap, S))
-            t_n = kept.sum(1)
-        o_key = t_key.cpu().numpy(); o_score = t_sbits.to(torch.int32).cpu().numpy().view(np.float32); o_tie = t_tie.to(torch.uint8).cpu().numpy(); o_n = t_n.cpu().numpy()
-        total = np.where(browse.cpu().numpy(), 0, o_n)          # (TotalCandidates is not set on the browse path)
-        self._acc("merge_sort_cut", tp); tp = time.perf_counter()
-        self.last_shard_info = M[:, :, 4:12]          # every shard's truncation facts of the last batch ([nq, W, 8]; diagnostics, tests)
-        total = np.where(whole, M[:, :, 1].sum(1).cpu().numpy(), total)      # TotalCandidates counts the whole list
-        facet_out = None
-        if facets:      # FacetBuilder over the records kept (one row per record and facetable column), or the summed rows of a whole Stage-1 list
-            nfc = len(self._fcols); fc = max(int(bufs["fcol"].shape[1]), 1)
-            cols = torch.tensor(self._fcols, dtype=torch.int32, device=self.dev).view(1, 1, nfc).expand(nq, cap, nfc)
-            ids = P[:, :, 1:]; cnt = ((pos_idx < t_n.view(nq, 1)).view(nq, cap, 1) & (ids >= 0)).to(torch.int32)
-            rows = torch.stack([cols, ids, cnt], 3).reshape(nq, cap * nfc, 3)
+        nq = len(queries); eng = self.eng
+        with self._timed(self.host_ms, "merge_pack"):
+            rec = np.zeros((nq, cap, 3), np.float64)          # key, score bits (exact in f64), tie
+            rec[:, :, 0] = bufs["keys"]; rec[:, :, 1] = bufs["scores"].view(np.uint32).astype(np.float64); rec[:, :, 2] = bufs["ties"]
+            meta = np.concatenate([np.stack([bufs["n"], bufs["total"], bufs["status"], bufs["nf"]], 1).astype(np.int64), bufs["info"].astype(np.int64), bufs["dkey"]], 1)      # [nq, 4 + 8 + 2]
+            t_rec = torch.from_numpy(rec).to(self.dev); t_meta = torch.from_numpy(meta).to(self.dev)
+            recs = [torch.empty_like(t_rec) for _ in range(W)]; metas = [torch.empty_like(t_meta) for _ in range(W)]
+            fq = np.array([q.EnableFacets for q in queries]); facets = bool(fq.any())
+        with self._timed(self.host_ms, "merge_gather"):
+            dist.all_gather(recs, t_rec); dist.all_gather(metas, t_meta)
+            if post is not None:
+                posts = [torch.empty_like(post) for _ in range(W)]; dist.all_gather(posts, post)
+            M = torch.stack(metas, 1)                                                                                                    # [nq, W, 14]
+            # a query answered with its WHOLE Stage-1 list (shard_info[6] == -1) was filtered on the shards: TotalCandidates and facet rows are summed
+            lst = (M[:, :, 10] == -1).cpu().numpy(); whole = lst.any(1)
+            sel = np.nonzero(whole & fq)[0]          # the same on every rank (from the gathered facts): each shard's facet rows of those queries
             if len(sel):
-                sr = torch.stack(srows, 1).reshape(len(sel), W * mine.shape[1], 3); m = max(rows.shape[1], sr.shape[1])
-                rows = torch.nn.functional.pad(rows, (0, 0, 0, m - rows.shape[1])).clone()
-                rows[torch.from_numpy(sel).to(self.dev)] = torch.nn.functional.pad(sr, (0, 0, 0, m - sr.shape[1]))
-            rows = rows.contiguous(); m = rows.shape[1]
-            f_col = torch.zeros((nq, fc), dtype=torch.int32, device=self.dev); f_val = torch.zeros_like(f_col); f_cnt = torch.zeros_like(f_col)
-            f_n = torch.zeros(nq, dtype=torch.int32, device=self.dev); st32 = status_t.to(torch.int32).contiguous()
-            p_ = lambda t: C.c_void_p(t.data_ptr())
-            eng._check(eng._gpu.ifx_batch_facet_table(h, p_(rows), m, p_(f_col), p_(f_val), p_(f_cnt), p_(f_n), p_(st32)), "ifx_batch_facet_table")
-            status_t = st32.to(torch.int64)
-            facet_out = (f_col.cpu().numpy(), f_val.cpu().numpy(), f_cnt.cpu().numpy(), f_n.cpu().numpy())
-        status = status_t.cpu().numpy()
-        status = np.where(whole & ~lst.all(1), status | 2, status)      # shards that disagree on the answer's kind: flagged, never mixed
-        self._acc("merge_facets", tp)
+                fr = np.stack([bufs["fcol"][sel], bufs["fval"][sel], np.where(np.arange(bufs["fcnt"].shape[1])[None, :] < bufs["nf"][sel, None], bufs["fcnt"][sel], 0)], 2).astype(np.int32)
+                mine = torch.from_numpy(np.ascontiguousarray(fr)).to(self.dev); srows = [torch.empty_like(mine) for _ in range(W)]; dist.all_gather(srows, mine)
+            self._sync()
+        with self._timed(self.host_ms, "merge_sort_cut"):
+            # merge on the device: ScoreEntry order (Score desc, Tiebreaker desc, DocumentId asc) = three stable sorts, least significant key first
+            R = torch.stack(recs, 1).reshape(nq, W * cap, 3)                                                                             # [nq, W*cap, 3]
+            valid = (torch.arange(cap, device=self.dev).view(1, 1, cap) < M[:, :, 0:1]).reshape(nq, W * cap)
+            key = R[:, :, 0].to(torch.int64); sbits = R[:, :, 1].to(torch.int64); tie = R[:, :, 2].to(torch.int64)
+            score = torch.where(valid, sbits.to(torch.int32).view(torch.float32).to(torch.float64), torch.full((), float("-inf"), dtype=torch.float64, device=self.dev))
+            o1 = torch.argsort(key, dim=1, stable=True)
+            o2 = torch.gather(o1, 1, torch.argsort(torch.gather(-tie, 1, o1), dim=1, stable=True))
+            order = torch.gather(o2, 1, torch.argsort(torch.gather(-score, 1, o2), dim=1, stable=True))[:, :cap]
+            # the blank query with EnableFacets (shard_info[6] == -2) browses the corpus in internal-id order: the shards' records in shard order
+            browse = (M[:, :, 10] == -2).any(1)
+            if bool(browse.any()):
+                order = torch.where(browse.view(nq, 1), torch.argsort((~valid).to(torch.int8), dim=1, stable=True)[:, :cap], order)
+            t_key = torch.gather(key, 1, order); t_sbits = torch.gather(sbits, 1, order); t_tie = torch.gather(tie, 1, order); nvalid = valid.sum(1)
+            maxr = torch.tensor([q.MaxNumberOfRecordsToReturn for q in queries], dtype=torch.int64, device=self.dev)
+            # ResultProcessor.CalculateTruncationIndex over the merged list: the last record with Score >= 254 (records are sorted: the first n_ge),
+            # or a docIndex-0/1 document whose word hits reach max(1, max word hits over all shards) or whose lcs is non-zero
+            info = M[:, :, 4:12]; dk = M[:, :, 12:14]
+            min_hits = info[:, :, 0].max(1).values.clamp(min=1); trunc = info[:, :, 1].sum(1) - 1
+            pos_idx = torch.arange(cap, device=self.dev).view(1, cap)
+            for j in range(2):
+                wh = info[:, :, 2 + 2 * j].max(1).values; lc = info[:, :, 3 + 2 * j].max(1).values; dkj = dk[:, :, j].max(1).values      # the owner reports >= 0, the others -1
+                qual = (wh >= 0) & ((wh >= min_hits) | (lc > 0))
+                hit = (t_key == dkj.view(nq, 1)) & (pos_idx < nvalid.clamp(max=cap).view(nq, 1))
+                pos = torch.where(hit.any(1), hit.to(torch.int64).argmax(1), torch.full((), cap, dtype=torch.int64, device=self.dev))      # beyond the merged top: at least `cap`
+                trunc = torch.where(qual, torch.maximum(trunc, pos), trunc)
+            count = torch.where(trunc < 0, maxr, torch.minimum(trunc + 1, maxr))
+            t_n = torch.minimum(torch.minimum(nvalid, count), maxr)
+            status_t = M[:, 0, 2].clone()
+            for r in range(1, W):
+                status_t |= M[:, r, 2]
+            P = None
+            if post is not None:      # ApplyFilter after the truncation: the records that fail leave, TotalCandidates counts the rest (Take(max) is then a no-op)
+                S = post.shape[2]
+                P = torch.gather(torch.stack(posts, 1).reshape(nq, W * cap, S), 1, order.unsqueeze(2).expand(nq, cap, S))
+                kept = (P[:, :, 0] == 1) & (pos_idx < t_n.view(nq, 1))
+                ko = torch.argsort((~kept).to(torch.int8), dim=1, stable=True)
+                t_key = torch.gather(t_key, 1, ko); t_sbits = torch.gather(t_sbits, 1, ko); t_tie = torch.gather(t_tie, 1, ko); P = torch.gather(P, 1, ko.unsqueeze(2).expand(nq, cap, S))
+                t_n = kept.sum(1)
+            o_key = t_key.cpu().numpy(); o_score = t_sbits.to(torch.int32).cpu().numpy().view(np.float32); o_tie = t_tie.to(torch.uint8).cpu().numpy(); o_n = t_n.cpu().numpy()
+            total = np.where(browse.cpu().numpy(), 0, o_n)          # (TotalCandidates is not set on the browse path)
+        with self._timed(self.host_ms, "merge_facets"):
+            self.last_shard_info = M[:, :, 4:12]          # every shard's truncation facts of the last batch ([nq, W, 8]; diagnostics, tests)
+            total = np.where(whole, M[:, :, 1].sum(1).cpu().numpy(), total)      # TotalCandidates counts the whole list
+            facet_out = None
+            if facets:      # FacetBuilder over the records kept (one row per record and facetable column), or the summed rows of a whole Stage-1 list
+                nfc = len(self._fcols); fc = max(int(bufs["fcol"].shape[1]), 1)
+                cols = torch.tensor(self._fcols, dtype=torch.int32, device=self.dev).view(1, 1, nfc).expand(nq, cap, nfc)
+                ids = P[:, :, 1:]; cnt = ((pos_idx < t_n.view(nq, 1)).view(nq, cap, 1) & (ids >= 0)).to(torch.int32)
+                rows = torch.stack([cols, ids, cnt], 3).reshape(nq, cap * nfc, 3)
+                if len(sel):
+                    sr = torch.stack(srows, 1).reshape(len(sel), W * mine.shape[1], 3); m = max(rows.shape[1], sr.shape[1])
+                    rows = torch.nn.functional.pad(rows, (0, 0, 0, m - rows.shape[1])).clone()
+                    rows[torch.from_numpy(sel).to(self.dev)] = torch.nn.functional.pad(sr, (0, 0, 0, m - sr.shape[1]))
+                rows = rows.contiguous(); m = rows.shape[1]
+                f_col = torch.zeros((nq, fc), dtype=torch.int32, device=self.dev); f_val = torch.zeros_like(f_col); f_cnt = torch.zeros_like(f_col)
+                f_n = torch.zeros(nq, dtype=torch.int32, device=self.dev); st32 = status_t.to(torch.int32).contiguous()
+                p_ = lambda t: C.c_void_p(t.data_ptr())
+                eng._check(eng._gpu.ifx_batch_facet_table(h, p_(rows), m, p_(f_col), p_(f_val), p_(f_cnt), p_(f_n), p_(st32)), "ifx_batch_facet_table")
+                status_t = st32.to(torch.int64)
+                facet_out = (f_col.cpu().numpy(), f_val.cpu().numpy(), f_cnt.cpu().numpy(), f_n.cpu().numpy())
+            status = status_t.cpu().numpy()
+            status = np.where(whole & ~lst.all(1), status | 2, status)      # shards that disagree on the answer's kind: flagged, never mixed
         self.last_raw = (o_key, o_score, o_tie, o_n, total, status)
         return o_key, o_score, o_tie, o_n, total, status, facet_out
 
-    def _results(self, queries, merged):
-        o_key, o_score, o_tie, o_n, total, status, facet_out = merged; out = []
-        for i, q in enumerate(queries):
-            records = [E.ScoreEntry(o_score[i, k], o_key[i, k], o_tie[i, k]) for k in range(int(o_n[i]))]
-            facets = None
-            if q.EnableFacets:
-                f_col, f_val, f_cnt, f_n = facet_out; facets = {}
-                for k in range(int(f_n[i])):
-                    col = int(f_col[i, k]); facets.setdefault(self.eng._columns[col], []).append((self.eng._facet_value(col, int(f_val[i, k])), int(f_cnt[i, k])))
-            out.append(E.Result(records, facets, int(total[i]), int(status[i])))
-        return out

@@ -434,31 +434,21 @@ class SearchEngine:
         """Batch form of Search: one C-ABI call for all queries (host buffers in, host buffers out)."""
         if not self._is_indexed:
             return [Result([], None, 0) for _ in queries]
-        nq = len(queries)
-        arr, keep = self._pack_queries(queries); post = self._pack_post(queries)
-        cap = max(1, max(q.MaxNumberOfRecordsToReturn for q in queries))
-        fc = facet_cap or (256 if any(q.EnableFacets for q in queries) else 0)
-        out = _BatchResult(); out.cap = cap; out.facet_cap = fc
-        keys = np.zeros((nq, cap), np.int64); scores = np.zeros((nq, cap), np.float32); ties = np.zeros((nq, cap), np.uint8)
-        n = np.zeros(nq, np.int32); total = np.zeros(nq, np.int32); status = np.zeros(nq, np.int32)
-        fcol = np.zeros((nq, max(fc, 1)), np.int32); fval = np.zeros((nq, max(fc, 1)), np.int32); fcnt = np.zeros((nq, max(fc, 1)), np.int32); nf = np.zeros(nq, np.int32)
-        out.doc_key, out.score, out.tie, out.n, out.total_candidates, out.status = _p(keys), _p(scores), _p(ties), _p(n), _p(total), _p(status)
-        out.facet_column, out.facet_value, out.facet_count, out.n_facets = _p(fcol), _p(fval), _p(fcnt), _p(nf)
-        st = stats if stats is not None else Stats()
-        if post is None:
-            self._check(self._gpu.ifx_search_batch(self._index, arr, nq, C.byref(out), C.byref(st)), "ifx_search_batch")
-        else:
-            self._check(self._gpu.ifx_search_batch_post(self._index, arr, post, nq, C.byref(out), C.byref(st)), "ifx_search_batch_post")
-        self.last_raw = (keys, scores, ties, n, total, status)
+        packed = self.PackBatch(queries, facet_cap); self.SearchPacked(packed, stats); b = packed["bufs"]
+        self.last_raw = (b["keys"], b["scores"], b["ties"], b["n"], b["total"], b["status"])
+        return self._results(queries, *self.last_raw, (b["fcol"], b["fval"], b["fcnt"], b["nf"]))
+
+    def _results(self, queries, keys, scores, ties, n, total, status, facets):
+        """Results of a batch from its per-query records, TotalCandidates, status and facet rows (column, value id, count, n_facets)."""
         res = []
-        for i in range(nq):
-            recs = [ScoreEntry(scores[i, k], keys[i, k], ties[i, k]) for k in range(n[i])]
-            facets = None
-            if queries[i].EnableFacets:
-                facets = {}
-                for k in range(nf[i]):
-                    facets.setdefault(self._columns[int(fcol[i, k])], []).append((self._facet_value(int(fcol[i, k]), int(fval[i, k])), int(fcnt[i, k])))
-            res.append(Result(recs, facets, int(total[i]), int(status[i])))
+        for i, q in enumerate(queries):
+            recs = [ScoreEntry(scores[i, k], keys[i, k], ties[i, k]) for k in range(int(n[i]))]
+            fs = None
+            if q.EnableFacets:
+                fcol, fval, fcnt, nf = facets; fs = {}
+                for k in range(int(nf[i])):
+                    col = int(fcol[i, k]); fs.setdefault(self._columns[col], []).append((self._facet_value(col, int(fval[i, k])), int(fcnt[i, k])))
+            res.append(Result(recs, fs, int(total[i]), int(status[i])))
         return res
 
     def _facet_value(self, col, vid):

@@ -54,11 +54,6 @@ def whole_list_batch(texts, three, flt):
     return batch(texts, flt, mx=500, coverage=False, blanks=False) + batch(three, flt, blanks=False) + batch(three[: len(three) // 2], flt, mx=600, blanks=False)
 
 
-def signature(r):
-    return ([(e.DocumentId, int(np.float32(e.Score).view(np.uint32)), int(e.Tiebreaker)) for e in r.Records], int(r.TotalCandidates), int(r.Status) & ~8,
-            None if r.Facets is None else {f: [(v, int(c)) for v, c in vs] for f, vs in r.Facets.items()})
-
-
 def oracle_signature(orc, q, flt_bytes):
     x = orc.search(q.Text, q.MaxNumberOfRecordsToReturn, coverage=q.EnableCoverage, filter_bytes=flt_bytes if q.Filter is not None else None, facets=q.EnableFacets)
     fo = None

@@ -81,9 +81,10 @@ def ngram_texts(vocab, n=24):
     return synth.gen_queries(n, synth.corpus_ref(N), vocab)
 
 
-def signature(r):
-    return ([(e.DocumentId, int(np.float32(e.Score).view(np.uint32)), int(e.Tiebreaker)) for e in r.Records], int(r.TotalCandidates), int(r.Status),
-            None if r.Facets is None else {f: list(v) for f, v in r.Facets.items()})
+def signature(r, ignore_status=0):
+    """(records, TotalCandidates, status without the flags `ignore_status`, facets) of a Result."""
+    return ([(e.DocumentId, int(np.float32(e.Score).view(np.uint32)), int(e.Tiebreaker)) for e in r.Records], int(r.TotalCandidates), int(r.Status) & ~ignore_status,
+            None if r.Facets is None else {f: [(v, int(c)) for v, c in vs] for f, vs in r.Facets.items()})
 
 
 def oracle_engine(keys, schema, cols):

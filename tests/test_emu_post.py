@@ -11,6 +11,7 @@ import pytest
 
 import infidex_b200 as ib
 import oracle_post
+from dist_util import spawn_gloo
 from infidex_b200 import synth
 from oracle import oracle as O
 from oracle.oracle import Field as OField
@@ -257,11 +258,9 @@ def test_host_builder_column_order(emu):
         mixed.Search(make_query("x", 10, sort=("v", True)))
 
 
-def _shard_worker(rank, world, port, emu, outdir):
+def _shard_worker(rank, world, emu, outdir):
     import pickle
     import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"; os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
     from infidex_b200 import dist as ifxd
     N = 140_000; vocab = synth.make_vocab(20_000)
     lo, hi = ifxd.shard_ranges(N, world)[rank]
@@ -277,17 +276,13 @@ def _shard_worker(rank, world, port, emu, outdir):
     if rank == 0:
         st = lambda rr: [r.Status for r in rr]
         pickle.dump((st(plain), st(boosted), st(sorted_), st(again)), open(os.path.join(outdir, "status.pkl"), "wb"))
-    dist.barrier(); dist.destroy_process_group()
 
 
 def test_sharded_index_flags_boosts_and_sort(tmp_path, emu):
     """Post-processing belongs after the hosts' merge of the shards, which is not built: on a 2-shard (gloo) index a query with boosts or a
     SortBy carries IFX_Q_UNSUPPORTED_OP; the others in the same batch do not."""
     import pickle
-    import socket
-    import torch.multiprocessing as mp
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
-    mp.spawn(_shard_worker, args=(2, port, emu, str(tmp_path)), nprocs=2, join=True)
+    spawn_gloo(_shard_worker, 2, emu, str(tmp_path))
     plain, boosted, sorted_, again = pickle.load(open(tmp_path / "status.pkl", "rb"))
     assert not any(x & 2 for x in plain) and not any(x & 2 for x in again)
     assert all(x & 2 for x in boosted)

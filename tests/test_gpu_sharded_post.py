@@ -1,8 +1,7 @@
 """Filters and facets on doc-id-range shards, on the GPU: two shard indexes in one process on one device, each rank's ShardedSearchEngine in its
-own thread, exchanging through a test-local stand-in for torch.distributed (CUDA tensors, a barrier). About a million multi-field documents
+own thread, exchanging through dist_util's stand-in for torch.distributed (CUDA tensors, a barrier). About a million multi-field documents
 and a 2 000-query batch with the C4 filter and facets (and the other variants of sharded_post_util), against the unsharded oracle with the
 acceptance rule; the uploaded and the packed paths of SearchBatch give identical answers."""
-import threading
 import time
 
 import numpy as np
@@ -12,73 +11,13 @@ import torch
 import infidex_b200 as ib
 
 import sharded_post_util as P
+import short_shard_util as U
+from dist_util import run_ranks
 
 pytestmark = pytest.mark.gpu
 
 N = 1_000_000
 NQ = 500          # texts; every one in the four variants of sharded_post_util: a batch of 2 003 queries
-
-
-class _Group:
-    def __init__(self, world):
-        self.world = world; self.slots = [None] * world; self.bar = threading.Barrier(world, timeout=600)
-
-
-class _ThreadDist:
-    """The part of torch.distributed that infidex_b200.dist uses, for ranks that are threads of one process."""
-
-    class ReduceOp:
-        SUM, MAX = "sum", "max"
-
-    def __init__(self, group, rank):
-        self.g, self.rank = group, rank
-
-    def get_rank(self):
-        return self.rank
-
-    def get_world_size(self):
-        return self.g.world
-
-    def _exchange(self, value):
-        self.g.slots[self.rank] = value
-        if torch.cuda.is_available():
-            torch.cuda.synchronize()
-        self.g.bar.wait(); vals = list(self.g.slots); self.g.bar.wait()
-        return vals
-
-    def barrier(self):
-        self.g.bar.wait()
-
-    def all_gather(self, out, t):
-        for o, v in zip(out, self._exchange(t.clone())):
-            o.copy_(v)
-
-    def all_reduce(self, t, op=ReduceOp.SUM):
-        vals = self._exchange(t.clone()); r = vals[0].clone()
-        for v in vals[1:]:
-            r = r + v if op == self.ReduceOp.SUM else torch.maximum(r, v)
-        t.copy_(r)
-
-    def all_gather_object(self, out, obj):
-        out[:] = self._exchange(obj)
-
-
-def _run_ranks(world, fn):
-    g = _Group(world); res = [None] * world; err = []
-
-    def body(r):
-        try:
-            res[r] = fn(_ThreadDist(g, r), r)
-        except BaseException as e:      # the other ranks would wait at the barrier forever
-            err.append(e); g.bar.abort()
-    ts = [threading.Thread(target=body, args=(r,)) for r in range(world)]
-    for t in ts:
-        t.start()
-    for t in ts:
-        t.join()
-    if err:
-        raise err[0]
-    return res
 
 
 def _docs(lo, hi, vocab):
@@ -100,7 +39,7 @@ def sharded():
         keys, schema, cols = _docs(*ranges[r], vocab)
         eng = ifxd.ShardedSearchEngine(d, device_index=0); eng.IndexShard(keys, schema, cols)
         return eng
-    engines = _run_ranks(2, build)
+    engines = run_ranks(2, build)
     keys, schema, cols = _docs(0, N, vocab)          # the unsharded oracle: the host builder's image of the whole corpus
     he = ib.SearchEngine.__new__(ib.SearchEngine); he._host = ib.engine._load_host(); he._builder = None; he._index = None; he._gpu = None
     he.IndexColumns(keys, schema, cols, upload=False)
@@ -121,8 +60,8 @@ def test_filters_and_facets_on_two_gpu_shards_match_the_unsharded_oracle(sharded
         torch.cuda.synchronize(); t0 = time.perf_counter()
         res = engines[r].SearchBatch(qs)
         torch.cuda.synchronize(); timing[r] = time.perf_counter() - t0
-        return [P.signature(x) for x in res]
-    a, b = _run_ranks(2, fn)
+        return [U.signature(x, ignore_status=8) for x in res]
+    a, b = run_ranks(2, fn)
     assert a == b          # every rank merges the same answer
     plain_bad, ids_bad, checked, bad = P.check(orc, qs, a, flt.bytecode())
     print("\n%s, two shards on one device: %d queries, %.1f ms per SearchBatch (both ranks' threads, exchanges and merge included); unfiltered "
@@ -142,8 +81,8 @@ def test_whole_stage1_lists_on_two_gpu_shards_match_the_unsharded_oracle(sharded
 
     def fn(d, r):
         engines[r].dist = d
-        return [P.signature(x) for x in engines[r].SearchBatch(qs)]
-    a, b = _run_ranks(2, fn)
+        return [U.signature(x, ignore_status=8) for x in engines[r].SearchBatch(qs)]
+    a, b = run_ranks(2, fn)
     assert a == b
     plain_bad, ids_bad, checked, bad = P.check(orc, qs, a, flt.bytecode())
     print("\nwhole-list queries: unfiltered records differ for %d of %d texts; %d filtered / faceted answers checked" % (plain_bad, len(qs) // 4, checked))
@@ -165,7 +104,7 @@ def test_uploaded_and_packed_batches_give_the_same_answers(sharded):
         finally:
             e.FreeBatch(up)
         via_packed = e.SearchBatch(qs, packed=e.eng.PackBatch(qs))
-        return [P.signature(x) for x in via_upload], [P.signature(x) for x in via_packed]
-    (u0, p0), (u1, p1) = _run_ranks(2, fn)
+        return [U.signature(x, ignore_status=8) for x in via_upload], [U.signature(x, ignore_status=8) for x in via_packed]
+    (u0, p0), (u1, p1) = run_ranks(2, fn)
     assert u0 == p0 == u1 == p1
     assert any(s[3] for s in u0)

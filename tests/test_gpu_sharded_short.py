@@ -1,79 +1,15 @@
 """Short queries on doc-id-range shards, on the GPU: two shard indexes in one process on one device, each rank's ShardedSearchEngine in its
-own thread, exchanging through a test-local stand-in for torch.distributed (CUDA tensors, a barrier). The same cases as the CPU test, a
+own thread, exchanging through dist_util's stand-in for torch.distributed (CUDA tensors, a barrier). The same cases as the CPU test, a
 batch large enough to take several groups of short queries, against the unsharded oracle; and the n-gram queries of a mixed batch against
 the same queries alone (the path without short queries)."""
-import threading
-
 import pytest
-import torch
 
 import infidex_b200 as ib
 
 import short_shard_util as U
+from dist_util import run_ranks
 
 pytestmark = pytest.mark.gpu
-
-
-class _Group:
-    def __init__(self, world):
-        self.world = world; self.slots = [None] * world; self.bar = threading.Barrier(world, timeout=600)
-
-
-class _ThreadDist:
-    """The part of torch.distributed that infidex_b200.dist uses, for ranks that are threads of one process."""
-
-    class ReduceOp:
-        SUM, MAX = "sum", "max"
-
-    def __init__(self, group, rank):
-        self.g, self.rank = group, rank
-
-    def get_rank(self):
-        return self.rank
-
-    def get_world_size(self):
-        return self.g.world
-
-    def _exchange(self, value):
-        self.g.slots[self.rank] = value
-        if torch.cuda.is_available():
-            torch.cuda.synchronize()
-        self.g.bar.wait(); vals = list(self.g.slots); self.g.bar.wait()
-        return vals
-
-    def barrier(self):
-        self.g.bar.wait()
-
-    def all_gather(self, out, t):
-        for o, v in zip(out, self._exchange(t.clone())):
-            o.copy_(v)
-
-    def all_reduce(self, t, op=ReduceOp.SUM):
-        vals = self._exchange(t.clone()); r = vals[0].clone()
-        for v in vals[1:]:
-            r = r + v if op == self.ReduceOp.SUM else torch.maximum(r, v)
-        t.copy_(r)
-
-    def all_gather_object(self, out, obj):
-        out[:] = self._exchange(obj)
-
-
-def _run_ranks(world, fn):
-    g = _Group(world); res = [None] * world; err = []
-
-    def body(r):
-        try:
-            res[r] = fn(_ThreadDist(g, r), r)
-        except BaseException as e:      # the other ranks would wait at the barrier forever
-            err.append(e); g.bar.abort()
-    ts = [threading.Thread(target=body, args=(r,)) for r in range(world)]
-    for t in ts:
-        t.start()
-    for t in ts:
-        t.join()
-    if err:
-        raise err[0]
-    return res
 
 
 @pytest.fixture(scope="module")
@@ -87,7 +23,7 @@ def sharded():
         eng = ifxd.ShardedSearchEngine(d, device_index=0)
         eng.IndexShard(keys[lo:hi], schema, [cols[0][lo:hi], cols[1][lo:hi]])
         return eng
-    engines = _run_ranks(2, build)
+    engines = run_ranks(2, build)
     yield engines, U.oracle_engine(keys, schema, cols), vocab
     for e in engines:
         e.Close()
@@ -97,7 +33,7 @@ def _search_with(engines, queries):
     def fn(d, r):
         engines[r].dist = d
         return [U.signature(x) for x in engines[r].SearchBatch(queries)]
-    a, b = _run_ranks(2, fn)
+    a, b = run_ranks(2, fn)
     assert a == b          # every rank merges the same answer
     return a
 

@@ -1,20 +1,14 @@
 """N > 1 host logic on CPU: two processes (gloo, world size 2), each with a replica of the index (kernel emulation build),
 rank-local query batches, max-over-ranks timing and the all-gather of result blocks."""
 import os
-import socket
 
 import numpy as np
-import pytest
+
+from dist_util import spawn_gloo
 
 
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
-
-
-def _worker(rank, world, port, emu, outdir):
+def _worker(rank, world, emu, outdir):
     import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"; os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
     import infidex_b200 as ib
     from infidex_b200 import dist as ifxd
     from infidex_b200 import synth
@@ -29,14 +23,11 @@ def _worker(rank, world, port, emu, outdir):
     np.save(os.path.join(outdir, "local_%d.npy" % rank), keys)
     if rank == 0:
         np.save(os.path.join(outdir, "gathered.npy"), np.stack(gathered)); np.save(os.path.join(outdir, "tmax.npy"), np.array(tmax))
-    dist.barrier(); dist.destroy_process_group()
 
 
 def test_two_rank_replicas(tmp_path):
-    import torch.multiprocessing as mp
     from parity_util import emu_lib
-    emu = emu_lib(); port = _free_port()
-    mp.spawn(_worker, args=(2, port, emu, str(tmp_path)), nprocs=2, join=True)
+    spawn_gloo(_worker, 2, emu_lib(), str(tmp_path))
     g = np.load(tmp_path / "gathered.npy"); l0 = np.load(tmp_path / "local_0.npy"); l1 = np.load(tmp_path / "local_1.npy")
     assert np.array_equal(g[0], l0) and np.array_equal(g[1], l1)
     assert not np.array_equal(l0, l1)                      # distinct batches per rank

@@ -3,20 +3,15 @@ exchanges of infidex_b200.dist.ShardedSearchEngine, and the merged result compar
 not exchanged (tier rules, threshold chain on shard-local counts; WordMatcher quota / truncation per shard) are allowed to show up as a small,
 counted number of differing queries -- the test pins that number's ceiling and that everything exchanged is exact."""
 import os
-import socket
 
 import numpy as np
 import pytest
 
-
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
+from dist_util import spawn_gloo
 
 
-def _worker(rank, world, port, emu, outdir, multi):
+def _worker(rank, world, emu, outdir, multi):
     import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"; os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
     import infidex_b200 as ib
     from infidex_b200 import dist as ifxd
     from infidex_b200 import synth
@@ -36,19 +31,16 @@ def _worker(rank, world, port, emu, outdir, multi):
     if rank == 0:
         import pickle
         pickle.dump([[(e.DocumentId, np.float32(e.Score).view(np.uint32).item(), e.Tiebreaker) for e in r.Records] for r in res], open(os.path.join(outdir, "merged.pkl"), "wb"))
-    dist.barrier(); dist.destroy_process_group()
 
 
 @pytest.mark.parametrize("multi", [False, True])
 def test_two_shards_against_the_unsharded_oracle(tmp_path, multi):
     import pickle
-    import torch.multiprocessing as mp
     from infidex_b200 import synth
     from oracle.oracle import Field as OField
     from oracle.oracle import OracleEngine
     from parity_util import emu_lib
-    emu = emu_lib(); port = _free_port()
-    mp.spawn(_worker, args=(2, port, emu, str(tmp_path), multi), nprocs=2, join=True)
+    spawn_gloo(_worker, 2, emu_lib(), str(tmp_path), multi)
     merged = pickle.load(open(tmp_path / "merged.pkl", "rb"))
     N = 180_000 if not multi else 140_000
     vocab = synth.make_vocab(30_000); docs = synth.gen_docs(N, vocab, with_description=multi)

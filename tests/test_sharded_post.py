@@ -7,7 +7,6 @@
     are not monotone in the internal id; and the short queries of short_shard_util that filter and count facets."""
 import ctypes as C
 import os
-import socket
 
 import numpy as np
 import pytest
@@ -17,6 +16,7 @@ from infidex_b200.engine import Field, Weight
 
 import sharded_post_util as P
 import short_shard_util as U
+from dist_util import run_ranks, spawn_gloo
 
 
 class _Strings(C.Structure):
@@ -85,21 +85,14 @@ def _builder(lo, hi, emu):
 
 @pytest.mark.parametrize("cuts", [[1_300], [700, 2_300], [1_000, 2_690]])
 def test_globalized_columns_equal_the_unsharded_dictionaries(cuts):
+    from infidex_b200.dist import exchange_builder
     from parity_util import emu_lib
     emu = emu_lib()
     want = _columns(_builder(0, N_A, emu))
     bounds = [0] + cuts + [N_A]; W = len(bounds) - 1
     shards = [_builder(bounds[s], bounds[s + 1], emu) for s in range(W)]
-    blobs = []
-    for e in shards:
-        ln = C.c_size_t(0); e._host.ifx_builder_export_columns.restype = C.c_void_p
-        p = e._host.ifx_builder_export_columns(C.c_void_p(e._builder), C.byref(ln))
-        blobs.append(np.ctypeslib.as_array((C.c_uint8 * ln.value).from_address(p)).copy())
-    arr = (C.c_void_p * W)(*[b.ctypes.data for b in blobs])
-    got = []
-    for s, e in enumerate(shards):
-        assert e._host.ifx_builder_globalize_columns(C.c_void_p(e._builder), W, s, arr) == 0
-        got.append(_columns(e))
+    run_ranks(W, lambda d, s: exchange_builder(d, shards[s], "ifx_builder_export_columns", "ifx_builder_globalize_columns"))
+    got = [_columns(e) for e in shards]
     for c, (vals, ids, rc, rank) in enumerate(want):
         for s in range(W):
             assert got[s][c][0] == vals, (c, s)                                            # the corpus's dictionary, unsharded order
@@ -107,10 +100,6 @@ def test_globalized_columns_equal_the_unsharded_dictionaries(cuts):
             assert got[s][c][2:] == (rc, rank), (c, s)                                     # the field's runtime kind over the corpus
     assert want[4][2] != 0 and want[0][2] == 0 and want[1][2] == 0         # the mixed field has no order; the int64 and double fields have one
     assert (want[3][1] == -1).any() and "" in want[2][0] and "1990" in want[0][0]      # nulls, an empty string, a value of the last shard only
-
-
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
 
 
 N_B = 140_000
@@ -127,11 +116,9 @@ def _short_cases():
     return [c for c in U.SHORT_CASES if c[2] or c[3]]
 
 
-def _worker(rank, world, port, emu, outdir):
+def _worker(rank, world, emu, outdir):
     import pickle
     import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"; os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
     from infidex_b200 import dist as ifxd
     from infidex_b200 import synth
     vocab = synth.make_vocab(30_000)
@@ -139,25 +126,23 @@ def _worker(rank, world, port, emu, outdir):
     keys, schema, cols = _synth_shard(lo, hi, vocab)
     eng = ifxd.ShardedSearchEngine(dist, _gpu_lib=emu); eng.IndexShard(keys, schema, cols, threads=2)
     flt = ib.Filter.Parse(P.C4_FILTER); texts = synth.gen_queries(80, synth.corpus_ref(N_B), vocab)
-    main = [P.signature(r) for r in eng.SearchBatch(P.batch(texts, flt))]
-    whole = [P.signature(r) for r in eng.SearchBatch(P.whole_list_batch(texts[:20], P.three_char_texts(vocab), flt))]
+    main = [U.signature(r, ignore_status=8) for r in eng.SearchBatch(P.batch(texts, flt))]
+    whole = [U.signature(r, ignore_status=8) for r in eng.SearchBatch(P.whole_list_batch(texts[:20], P.three_char_texts(vocab), flt))]
     eng.Close()
     skeys, sschema, scols, _ = U.corpus()
     lo, hi = ifxd.shard_ranges(U.N, world)[rank]
     seng = ifxd.ShardedSearchEngine(dist, _gpu_lib=emu); seng.IndexShard(skeys[lo:hi], sschema, [scols[0][lo:hi], scols[1][lo:hi]], threads=2)
-    short = [P.signature(r) for r in seng.SearchBatch([U.make_query(c) for c in _short_cases()])]
+    short = [U.signature(r, ignore_status=8) for r in seng.SearchBatch([U.make_query(c) for c in _short_cases()])]
     seng.Close()
     if rank == 0:
         pickle.dump({"main": main, "whole": whole, "short": short}, open(os.path.join(outdir, "out.pkl"), "wb"))
-    dist.barrier(); dist.destroy_process_group()
 
 
 def test_two_shards_filter_and_count_facets_as_the_unsharded_oracle(tmp_path):
     import pickle
-    import torch.multiprocessing as mp
     from infidex_b200 import synth
     from parity_util import emu_lib
-    mp.spawn(_worker, args=(2, _free_port(), emu_lib(), str(tmp_path)), nprocs=2, join=True)
+    spawn_gloo(_worker, 2, emu_lib(), str(tmp_path))
     out = pickle.load(open(tmp_path / "out.pkl", "rb"))
     vocab = synth.make_vocab(30_000)
     keys, schema, cols = _synth_shard(0, N_B, vocab)

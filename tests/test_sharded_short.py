@@ -5,7 +5,6 @@ The search path on CPU: two processes (gloo, world size 2), each holding one sha
 built from its own index: ids, score bits, tiebreakers, TotalCandidates and status (a shard's batch carries no facet tables)."""
 import ctypes as C
 import os
-import socket
 
 import numpy as np
 import pytest
@@ -15,6 +14,7 @@ from infidex_b200 import synth
 from infidex_b200.engine import Field, Weight
 
 import short_shard_util as U
+from dist_util import run_ranks, spawn_gloo
 
 
 class _Strings(C.Structure):
@@ -59,6 +59,7 @@ def _tie_corpus():
 
 @pytest.mark.parametrize("cuts", [[3_000], [3_000, 6_000], [2_980, 6_010]])
 def test_globalized_champions_equal_the_unsharded_lists(cuts):
+    from infidex_b200.dist import exchange_builder
     keys, titles = _tie_corpus(); n = len(keys)
     schema = [Field("title", None, Weight.High)]
     whole = ib.SearchEngine(); whole.IndexColumns(keys, schema, [titles], upload=False)
@@ -67,16 +68,8 @@ def test_globalized_champions_equal_the_unsharded_lists(cuts):
     shards = []
     for s in range(W):
         e = ib.SearchEngine(); e.IndexColumns(keys[bounds[s]:bounds[s + 1]], schema, [titles[bounds[s]:bounds[s + 1]]], upload=False); shards.append(e)
-    blobs = []
-    for e in shards:
-        ln = C.c_size_t(0); e._host.ifx_builder_export_champions.restype = C.c_void_p
-        p = e._host.ifx_builder_export_champions(C.c_void_p(e._builder), C.byref(ln))
-        blobs.append(np.ctypeslib.as_array((C.c_uint8 * ln.value).from_address(p)).copy())
-    arr = (C.c_void_p * W)(*[b.ctypes.data for b in blobs])
-    got = []
-    for s, e in enumerate(shards):
-        assert e._host.ifx_builder_globalize_champions(C.c_void_p(e._builder), W, s, arr) == 0
-        got.append(_champions(e))
+    run_ranks(W, lambda d, s: exchange_builder(d, shards[s], "ifx_builder_export_champions", "ifx_builder_globalize_champions"))
+    got = [_champions(e) for e in shards]
     tied = 0
     for ch, (doc, score) in want.items():
         glob = np.full(len(doc), -1, np.int64)
@@ -91,15 +84,9 @@ def test_globalized_champions_equal_the_unsharded_lists(cuts):
         assert set(got[s]) == set(want)
 
 
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
-
-
-def _worker(rank, world, port, emu, outdir):
+def _worker(rank, world, emu, outdir):
     import pickle
     import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"; os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
     from infidex_b200 import dist as ifxd
     keys, schema, cols, vocab = U.corpus()
     lo, hi = ifxd.shard_ranges(U.N, world)[rank]
@@ -112,14 +99,12 @@ def _worker(rank, world, port, emu, outdir):
     eng.Close()
     if rank == 0:
         pickle.dump({"alone": alone, "mixed": mixed, "counts": counts, "info": info}, open(os.path.join(outdir, "out.pkl"), "wb"))
-    dist.barrier(); dist.destroy_process_group()
 
 
 def test_two_shards_answer_short_queries_as_the_unsharded_oracle(tmp_path):
     import pickle
-    import torch.multiprocessing as mp
     from parity_util import emu_lib
-    mp.spawn(_worker, args=(2, _free_port(), emu_lib(), str(tmp_path)), nprocs=2, join=True)
+    spawn_gloo(_worker, 2, emu_lib(), str(tmp_path))
     out = pickle.load(open(tmp_path / "out.pkl", "rb"))
     ns = len(U.SHORT_CASES)
     assert out["mixed"][ns:] == out["alone"]                    # the n-gram queries of a mixed batch are untouched

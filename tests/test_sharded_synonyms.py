@@ -6,15 +6,13 @@ import pickle
 
 import numpy as np
 
-from test_sharded import _free_port
+from dist_util import spawn_gloo
 
 N = 160_000
 
 
-def _worker(rank, world, port, emu, outdir):
+def _worker(rank, world, emu, outdir):
     import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"; os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
     import infidex_b200 as ib
     from infidex_b200 import dist as ifxd
     from infidex_b200 import synth
@@ -30,7 +28,6 @@ def _worker(rank, world, port, emu, outdir):
     eng.Close()
     if rank == 0:
         pickle.dump([[(e.DocumentId, np.float32(e.Score).view(np.uint32).item(), e.Tiebreaker) for e in r.Records] for r in res], open(os.path.join(outdir, "merged.pkl"), "wb"))
-    dist.barrier(); dist.destroy_process_group()
 
 
 def _queries(vocab):
@@ -41,13 +38,11 @@ def _queries(vocab):
 
 
 def test_two_shards_with_a_map_against_the_unsharded_oracle(tmp_path):
-    import torch.multiprocessing as mp
     from infidex_b200 import synth
     from oracle.oracle import Field as OField
     from oracle_syn import SynOracleEngine
     from parity_util import emu_lib
-    emu = emu_lib(); port = _free_port()
-    mp.spawn(_worker, args=(2, port, emu, str(tmp_path)), nprocs=2, join=True)
+    spawn_gloo(_worker, 2, emu_lib(), str(tmp_path))
     merged = pickle.load(open(tmp_path / "merged.pkl", "rb"))
     vocab = synth.make_vocab(30_000); docs = synth.gen_docs(N, vocab)
     schema, cols = synth.schema_and_columns(docs, False)

@@ -1,7 +1,8 @@
 """Cost of answering short queries (no word of >= 3 characters) on doc-id-range shards.
 
-1. Build time (CPU, host builder only): the champion exchange of a corpus split 2 and 8 ways -- bytes all-gathered and the seconds of one
-   shard's ifx_builder_export_champions and ifx_builder_globalize_champions (shards export in parallel on their own hosts).
+1. Build time (CPU, host builder only): the champion exchange of a corpus split 2 and 8 ways -- bytes all-gathered and the seconds of the
+   slowest shard's ifx_builder_export_champions, all-gather and ifx_builder_globalize_champions (every shard's builder a thread of this
+   process, so the shards share this host's cores).
 2. Search (GPU): ms per batch of a short-heavy batch, two shards on one device through the in-process harness (each rank a thread,
    exchanging through CUDA tensors), against the unsharded engine on the same corpus. Under torchrun with >= 2 GPUs the shards run one per
    GPU over NCCL instead.
@@ -10,18 +11,18 @@
     torchrun --nproc-per-node 2 tools/bench_sharded_short.py --skip-build
 """
 import argparse
-import ctypes as C
 import json
 import os
 import sys
-import threading
 import time
 
 import numpy as np
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import infidex_b200 as ib                      # noqa: E402
+from dist_util import run_ranks                # noqa: E402
 from infidex_b200 import dist as ifxd          # noqa: E402
 from infidex_b200 import synth                 # noqa: E402
 
@@ -34,88 +35,22 @@ def short_batch(n_ngram_texts):
 
 
 def build_exchange(n_docs, world, threads):
-    """Bytes and seconds of the champion exchange at `world` shards (one shard's builder timed; blobs of all shards)."""
+    """Bytes and seconds of the champion exchange at `world` shards (all shards' builders at once, the slowest shard timed)."""
     vocab = synth.make_vocab(100_000)
     schema = [ib.Field("title", None, ib.Weight.Med)]
-    blobs, t_export, keep = [], [], None
-    for r, (lo, hi) in enumerate(ifxd.shard_ranges(n_docs, world)):
+    shards = []
+    for lo, hi in ifxd.shard_ranges(n_docs, world):
         docs = synth.gen_docs(hi - lo, vocab, start=lo)
-        e = ib.SearchEngine(); e.IndexColumns(docs["keys"], schema, [docs["title"]], threads=threads, upload=False)
-        ln = C.c_size_t(0); e._host.ifx_builder_export_champions.restype = C.c_void_p
-        t0 = time.perf_counter(); p = e._host.ifx_builder_export_champions(C.c_void_p(e._builder), C.byref(ln)); t_export.append(time.perf_counter() - t0)
-        blobs.append(np.ctypeslib.as_array((C.c_uint8 * ln.value).from_address(p)).copy())
-        if r == 0:
-            keep = e
-        else:
-            e.Dispose()
-    arr = (C.c_void_p * world)(*[b.ctypes.data for b in blobs])
-    t0 = time.perf_counter(); rc = keep._host.ifx_builder_globalize_champions(C.c_void_p(keep._builder), world, 0, arr); t_glob = time.perf_counter() - t0
-    assert rc == 0
-    keep.Dispose()
-    return {"docs": n_docs, "shards": world, "exchange_bytes": int(sum(len(b) for b in blobs)), "export_s_max": round(max(t_export), 3),
-            "globalize_s": round(t_glob, 3)}
+        e = ib.SearchEngine(); e.IndexColumns(docs["keys"], schema, [docs["title"]], threads=threads, upload=False); shards.append(e)
 
-
-class _Group:
-    def __init__(self, world):
-        self.world = world; self.slots = [None] * world; self.bar = threading.Barrier(world, timeout=600)
-
-
-class ThreadDist:
-    """torch.distributed's collectives for ranks that are threads of one process (CUDA tensors on one device)."""
-
-    class ReduceOp:
-        SUM, MAX = "sum", "max"
-
-    def __init__(self, group, rank):
-        self.g, self.rank = group, rank
-
-    def get_rank(self):
-        return self.rank
-
-    def get_world_size(self):
-        return self.g.world
-
-    def _exchange(self, value):
-        import torch
-        self.g.slots[self.rank] = value; torch.cuda.synchronize()
-        self.g.bar.wait(); vals = list(self.g.slots); self.g.bar.wait()
-        return vals
-
-    def barrier(self):
-        self.g.bar.wait()
-
-    def all_gather(self, out, t):
-        for o, v in zip(out, self._exchange(t.clone())):
-            o.copy_(v)
-
-    def all_reduce(self, t, op=ReduceOp.SUM):
-        import torch
-        vals = self._exchange(t.clone()); r = vals[0].clone()
-        for v in vals[1:]:
-            r = r + v if op == self.ReduceOp.SUM else torch.maximum(r, v)
-        t.copy_(r)
-
-    def all_gather_object(self, out, obj):
-        out[:] = self._exchange(obj)
-
-
-def run_ranks(world, fn):
-    g = _Group(world); res = [None] * world; err = []
-
-    def body(r):
-        try:
-            res[r] = fn(ThreadDist(g, r), r)
-        except BaseException as e:
-            err.append(e); g.bar.abort()
-    ts = [threading.Thread(target=body, args=(r,)) for r in range(world)]
-    for t in ts:
-        t.start()
-    for t in ts:
-        t.join()
-    if err:
-        raise err[0]
-    return res
+    def fn(d, r):
+        t0 = time.perf_counter()
+        blobs = ifxd.exchange_builder(d, shards[r], "ifx_builder_export_champions", "ifx_builder_globalize_champions")
+        return time.perf_counter() - t0, sum(len(b) for b in blobs)
+    res = run_ranks(world, fn)
+    for e in shards:
+        e.Dispose()
+    return {"docs": n_docs, "shards": world, "exchange_bytes": int(res[0][1]), "exchange_s_max": round(max(t for t, _ in res), 3)}
 
 
 def time_batches(fn, steps, warmup):
