@@ -35,7 +35,8 @@ enum {
 /* per-query status bits in ifx_batch_result.status */
 enum {
     IFX_Q_OK = 0,
-    IFX_Q_UNSUPPORTED_OP = 2, /* MATCHES (regex) opcode; a query without a word of >= 3 characters over documents that share a DocumentKey */
+    IFX_Q_UNSUPPORTED_OP = 2, /* MATCHES (regex) opcode; a query without a word of >= 3 characters on a doc-id-range shard whose documents
+                                 share a DocumentKey (one GPU answers those) */
     IFX_Q_OVERFLOW = 4,       /* a fixed device buffer was too small for this query */
     IFX_Q_EMPTY = 8           /* blank query -> empty result (SearchEngine.cs:295-296) */
 };

@@ -6,7 +6,8 @@
 //                                                                                                           fuzzy fallback over ALL terms, final scores)
 // Such queries are rare and touch the whole corpus by construction, so each one runs as a few grid-wide launches over per-index scratch arrays
 // (an int and a float per document) instead of inside the per-CTA pipeline; the result is the same Stage-1 list (doc, score, key; score
-// descending, key ascending) the rest of the pipeline consumes, plus the number of matched documents (Result.TotalCandidates).
+// descending, key ascending) the rest of the pipeline consumes, plus the number of matched documents (Result.TotalCandidates). Where
+// DocumentKeys repeat, all of it is per key (sq_slot).
 // Written against ifx::Ctx like everything else: `blk` / `nblk` stand for blockIdx / gridDim so the test build can run the same code.
 #pragma once
 #include "ifx_stage1.h"
@@ -18,8 +19,23 @@ constexpr int SQ_KB = 1024;           // top-K capacity of the selection (>= dep
 constexpr int SQ_TERMS = 4096;        // ShortQueryProcessor: terms collected per prefix pattern
 constexpr int SQ_PATTERNS = 4;
 
-struct SqScratch { int32_t* vi; float* vf; int32_t* terms; int32_t* tmult; int32_t* counters;       // counters: [0] matched documents, [1] term-list length, [2] max int score, [3] total with score > 0
-                   float* cand_score; int64_t* cand_key; int32_t* cand_doc; int32_t* cand_n; };    // [nblk][SQ_KB] per-block survivors of the selection
+struct SqScratch { int32_t* vi; float* vf; int32_t* terms; int32_t* tmult; int32_t* counters;       // counters: [0] matched keys, [1] term-list length, [2] max int score, [3] total with score > 0
+                   float* cand_score; int64_t* cand_key; int32_t* cand_doc; int32_t* cand_n;      // [nblk][SQ_KB] per-block survivors of the selection
+                   uint32_t* seen; uint32_t* kpre; };     // repeated keys only (null otherwise): bit per document "in a processed posting list",
+                                                          // bit per key slot "some matched segment's text starts with the query"
+// Repeated DocumentKeys (ix.key_first non-null): the reference accumulates SearchShortQuery per KEY and consolidates the other paths per key
+// (ShortQueryProcessor.cs:281-296,355-380, SegmentProcessor.cs:15-37). Every per-key quantity lives in the slot of the key's first live
+// document, key_first[d]; the other documents' slots stay 0, so the selection below never sees two entries of one key.
+IFX_FN int sq_slot(const DevIndex& ix, int doc) { return ix.key_first ? ix.key_first[doc] : doc; }
+IFX_FN bool sq_bit(const uint32_t* b, int i) { return (b[i >> 5] >> (i & 31)) & 1u; }
+// vf[slot] = max(vf[slot], s) for s > 0: positive floats order as their bit patterns
+IFX_FN void sq_max_into(float* p, float s) {
+#ifdef IFX_EMU
+    int v; memcpy(&v, &s, 4); atomic_max(reinterpret_cast<int*>(p), v);
+#else
+    atomic_max(reinterpret_cast<int*>(p), __float_as_int(s));
+#endif
+}
 
 // ToLowerInvariant(IndexedText) of one document: the raw text where it differs from the normalised one, else the normalised text
 IFX_FN void sq_doc_text(const DevIndex& ix, int doc, const uint16_t*& p, int& n) {
@@ -72,12 +88,20 @@ IFX_FN void sq_collect_pattern_terms(const DevIndex& ix, const SqPatterns& P, Sq
     }
     S.counters[1] = nt;
 }
-// ProcessTermMatches over one term: score[doc] += weight * mult for every live document of its posting list (one warp per term)
+// ProcessTermMatches over one term: score[key] += weight * mult for every live document of its posting list (one warp per term)
 IFX_FN void sq_process_term(const Ctx& c, const DevIndex& ix, int ord, int mult, SqScratch S) {
     if (ix.df[ord] <= 0) return;
     const int64_t r0 = ix.row_ptr[ord], r1 = ix.row_ptr[ord + 1];
     for (int64_t i = r0 + c.lane(); i < r1; i += Ctx::WS) { const int d = ix.post_doc[i]; if (ix.deleted[d]) continue;
-        const int old = atomic_add(&S.vi[d], (int)ix.post_tf[i] * mult); if (old == 0) atomic_add(&S.counters[0], 1); }
+        const int old = atomic_add(&S.vi[sq_slot(ix, d)], (int)ix.post_tf[i] * mult); if (old == 0) atomic_add(&S.counters[0], 1);
+        if (S.seen && !sq_bit(S.seen, d)) atomic_or(&S.seen[d >> 5], 1u << (d & 31)); }
+}
+// ToLowerInvariant(IndexedText).StartsWith(searchLower) of one document (ProcessTermMatches, ShortQueryProcessor.cs:281-296)
+IFX_FN bool sq_first_prefix(const DevIndex& ix, int doc, const uint16_t* q, int qlen) {
+    const uint16_t* t; int n; sq_doc_text(ix, doc, t, n);
+    if (n < qlen) return false;
+    for (int k = 0; k < qlen; k++) if (lo_c(ix, t[k]) != q[k]) return false;
+    return true;
 }
 // ProcessFuzzyFallback (matched < 100): every dictionary term that does not start with a pattern and holds a query character
 IFX_FN int sq_fuzzy_weight(const DevIndex& ix, int ord, const SqPatterns& P, const uint16_t* q, int qlen) {
@@ -89,8 +113,9 @@ IFX_FN int sq_fuzzy_weight(const DevIndex& ix, int ord, const SqPatterns& P, con
         if (wb) { boundary = true; cm++; } else if (any) cm++; }
     return (boundary || cm > 0) ? (boundary ? 2 : 1) : 0;
 }
-// BuildFinalScores / ComputePrecedence for one matched document
-IFX_FN float sq_final_score(const DevIndex& ix, int doc, int v, int vmax, const uint16_t* q, int qlen) {
+// BuildFinalScores / ComputePrecedence for one matched key, read from its first live document `doc`. `key_prefix`: the key's first-token-prefix
+// flag when keys repeat (taken from whichever segment matched), -1 to read it from `doc` itself
+IFX_FN float sq_final_score(const DevIndex& ix, int doc, int v, int vmax, const uint16_t* q, int qlen, int key_prefix) {
     const float normalized = vmax > 0 ? (float)v / (float)vmax : (float)v / 255.f;
     const uint16_t* t; int n; sq_doc_text(ix, doc, t, n);
     // query tokens
@@ -113,7 +138,7 @@ IFX_FN float sq_final_score(const DevIndex& ix, int doc, int v, int vmax, const 
             n_words++; }
         int tb = 0, te = n; while (tb < te && sq_is_ws(ix, lo_c(ix, t[tb]))) tb++; while (te > tb && sq_is_ws(ix, lo_c(ix, t[te - 1]))) te--;
         const bool title_eq = word_eq(tb, te, q, qlen);
-        bool first_prefix = n >= qlen; for (int k = 0; k < qlen && first_prefix; k++) if (lo_c(ix, t[k]) != q[k]) first_prefix = false;
+        const bool first_prefix = key_prefix >= 0 ? key_prefix != 0 : sq_first_prefix(ix, doc, q, qlen);
         if (any_exact) prec |= 1; if (first_prefix) prec |= 2; if (first_exact) prec |= 4; if (title_eq) prec |= 8;
     }
     return (float)prec + normalized;
@@ -162,13 +187,19 @@ IFX_FN void sq_topk_stage2(const Ctx& c, SqScratch S, SqTopShared& sh, int nblk,
 }
 // champion path (one character, max_results <= 64, list long enough): TopKHeap(max) over the first `max` champions, consolidated order.
 // On a doc-id-range shard the lists are the global ones and another shard's entries are -1: only this shard's entries among the first `max`
-// are written (the hosts' global cut merges them).
+// are written (the hosts' global cut merges them). Repeated keys: the champions are documents, so the best entry per key is kept
+// (ConsolidateSegments after Take(max): the list can be shorter than `max`) and it hands the key's first live document on.
 IFX_FN void sq_champions(const Ctx& c, const DevIndex& ix, SqTopShared& sh, int ci, int m, int64_t* out_key, int32_t* out_doc, float* out_score, int32_t* out_n, int32_t* out_total) {
     sq_clear(c, sh, 0, 128); const int b = ix.champ_off[ci];
     for (int i = c.tid(); i < m; i += c.nthreads()) { const int d = ix.champ_doc[b + i]; if (d < 0) continue; sh.score[i] = ix.champ_score[b + i]; sh.doc[i] = d; sh.key[i] = ix.doc_key[d]; }
     c.sync();
     if (c.tid() == 0) { int own = 0; for (int i = 0; i < m; i++) own += ix.champ_doc[b + i] >= 0; sh.bcast[0] = own; }
     sq_sort_desc(c, sh, 128);
+    if (ix.key_first && c.tid() == 0) { int kept = 0;
+        for (int i = 0; i < sh.bcast[0]; i++) { bool seen = false; for (int j = 0; j < kept && !seen; j++) seen = sh.key[j] == sh.key[i];
+            if (!seen) { sh.score[kept] = sh.score[i]; sh.key[kept] = sh.key[i]; sh.doc[kept] = ix.key_first[sh.doc[i]]; kept++; } }
+        sh.bcast[0] = kept; }
+    c.sync();
     const int own = sh.bcast[0];
     for (int i = c.tid(); i < own; i += c.nthreads()) { out_key[i] = sh.key[i]; out_doc[i] = sh.doc[i]; out_score[i] = sh.score[i]; }
     if (c.tid() == 0) { out_n[0] = own; out_total[0] = own; }

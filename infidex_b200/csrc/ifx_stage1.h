@@ -50,12 +50,11 @@ IFX_FN void prepare_query(const DevIndex& ix, const uint16_t* text, int len, int
     }
     bool can_ngrams = n_words == 0 ? len >= 3 : n_long > 0;
     if (!can_ngrams) {      // no word of >= 3 characters: ShortQueryProcessor / ShortQueryResolver (SearchPipeline.cs:222-262), scored by the launches of ifx_short.h
-        // documents sharing a DocumentKey (the reference accumulates short-query scores per KEY): that combination is not built -- flagged
-        // (IFX_Q_UNSUPPORTED_OP), never answered partially. A shard keeps the query's kind, so every shard counts the same short queries
-        // (the hosts' exchange rounds, ifx_batch_short_groups).
-        if (ix.key_first && !ix.prefix_gcard) { p.status |= 2; return; }
+        // documents sharing a DocumentKey are accumulated and consolidated per key (ifx_short.h sq_slot). On a doc-id-range shard a key's
+        // segments may sit on two shards, whose per-key partial sums nothing exchanges: flagged (IFX_Q_UNSUPPORTED_OP), never answered
+        // partially. The shard keeps the query's kind, so every shard counts the same short queries (the hosts' exchange rounds, ifx_batch_short_groups).
         p.short_kind = len == 1 ? 1 : 2; p.tlen = 0;
-        if (ix.key_first) { p.status |= 2; return; }
+        if (ix.key_first && ix.prefix_gcard) { p.status |= 2; return; }
         bool short3 = len <= 3; for (int i = 0; i < len; i++) if (is_delim(ix, text[i])) short3 = false;
         p.is_short3 = short3; int64_t pc = -1;
         if (short3) { int k = dict_lookup(ix.prefix.keys, text, len); pc = k < 0 ? 0 : (ix.prefix_gcard ? (int64_t)ix.prefix_gcard[k] : ix.prefix.row_ptr[k + 1] - ix.prefix.row_ptr[k]); if (pc > 500) p.short_skip_coverage = 1; }

@@ -461,7 +461,8 @@ IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p,
         c.sync();
         for (int i = c.tid(); i < n2; i += NT) if (sh.idx[i] >= 0) sh.pos[sh.idx[i]] = i;
         c.sync();
-        // TopKHeap(K) keeps the K best entries; ConsolidateSegments keeps the better of two entries with the same key.
+        // TopKHeap(K) keeps the K best entries; ConsolidateSegments keeps the better of two entries with the same key, and the filter, boosts,
+        // SortBy and facets read the key's first live document (GetDocumentByPublicKey), whichever segment the entry came from.
         // Valid entries sort in front of the invalid ones, so "the first K valid positions" is a prefix: per-position keep flags
         // and an ordered compaction, round by round.
         const int lim = n2 < K ? n2 : K; int nk = 0;
@@ -470,7 +471,7 @@ IFX_FN void finalize_query(const Ctx& c, const DevIndex& ix, const QueryPlan& p,
             if (i < lim) { e = sh.idx[i]; if (e >= 0) { int tw = B.ent_twin[eo + e]; keep = !(tw >= 0 && sh.pos[tw] < i);
                 if (keep && ix.key_first) { const int64_t k = sh.ekey[e]; for (int j = 0; j < i && keep; j++) { const int ej = sh.idx[j]; if (ej >= 0 && sh.ekey[ej] == k) keep = false; } } } }      // duplicate keys: the better entry of a key wins
             int tot; int off = block_excl_scan(c, keep ? 1 : 0, sh.scan, tot);
-            if (keep) { sh.keep_doc[nk + off] = B.ent_doc[eo + e]; sh.keep_score[nk + off] = sh.score[i]; sh.keep_tie[nk + off] = sh.etie[e]; }
+            if (keep) { const int d = B.ent_doc[eo + e]; sh.keep_doc[nk + off] = ix.key_first ? ix.key_first[d] : d; sh.keep_score[nk + off] = sh.score[i]; sh.keep_tie[nk + off] = sh.etie[e]; }
             nk += tot;
         }
         // ResultProcessor.CalculateTruncationIndex: only docIndex 0/1 have stored word hits / lcs (Span2D height-2 quirk): for each of
